@@ -374,9 +374,8 @@ struct Driver {
 		// float mantissa keeps them multiples of 2^-32 in any realistic range, so the reference's double arithmetic is exact
 		// and a 2^-32 fixed-point integer reproduces it; the double loop below remains as the fallback when a gap penalty is
 		// not representable.
-		static const bool no_fixed = getenv("MM_B200_NO_FIXED_EXTRA") != nullptr; // debugging aid: force the double loop
-		bool fixed_ok = !no_fixed;
-		if (fixed_ok) {
+		bool fixed_ok = true;
+		{
 			int64_t matfx[25];
 			for (int i = 0; i < 25; ++i) matfx[i] = (int64_t)mat[i] << 32;
 			int64_t sfx = 0, maxfx = 0;
@@ -651,10 +650,9 @@ struct Driver {
 		}
 		// What follows up to the gap-fill list depends on the anchors only (spliced reads: and on the end probes, which are awaited first):
 		// it is computed by the first replay that gets this far and kept in the read's plan list; later replays start at the extensions.
-		static const bool no_plan = getenv("MM_B200_NO_PLAN_CACHE") != nullptr; // development switch: plan every hit in every replay
 		const int32_t key_as = r->as, key_cnt = r->cnt;
 		HlHitPlan *P = nullptr;
-		if (!no_plan) for (HlHitPlan &hp : ra.plans) if (hp.as == key_as && hp.cnt == key_cnt && hp.splice_flag == (splice_flag << 1 | (r->split_inv? 1 : 0))) { P = &hp; break; }
+		for (HlHitPlan &hp : ra.plans) if (hp.as == key_as && hp.cnt == key_cnt && hp.splice_flag == (splice_flag << 1 | (r->split_inv? 1 : 0))) { P = &hp; break; }
 		HlHitPlan fresh; // used when the hit has no stored plan yet
 		if (P) {
 			as1 = P->as1, cnt1 = P->cnt1, rs = P->rs, qs = P->qs, re = P->re, qe = P->qe, rs0 = P->rs0, qs0 = P->qs0, re0 = P->re0, qe0 = P->qe0;
@@ -749,7 +747,8 @@ struct Driver {
 					}
 				}
 			}
-			if (!no_plan) { ra.plans.push_back(std::move(fresh)); P = &ra.plans.back(); } else P = &fresh;
+			ra.plans.push_back(std::move(fresh));
+			P = &ra.plans.back();
 		} // planning
 
 		// left extension (align.c:779-799)

@@ -744,11 +744,10 @@ void mmb_ksw_launch(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, int n_jobs, const
 	std::vector<std::vector<int>> tj(2 * (n_tiers + 1)); // [0, n_tiers]: ksw_extd2 jobs, [n_tiers+1, ..]: spliced (ksw_exts2) jobs
 	uint64_t cells = 0, io_bytes = 0;
 	std::vector<int> llj, fastj;
-	static const bool use_fast = getenv("MM_B200_NO_FAST_KSW") == nullptr;
 	for (int i = 0; i < n_jobs; ++i) {
 		if (h_jobs[i].flag & MMB_JOB_LL) { llj.push_back(i); continue; }
 		const bool spl = (h_jobs[i].flag & MMB_JOB_SPLICE) != 0;
-		if (use_fast && !spl && mmb_ksw_fast_eligible(h_jobs[i])) {
+		if (!spl && mmb_ksw_fast_eligible(h_jobs[i])) {
 			fastj.push_back(i);
 			cells += (uint64_t)h_jobs[i].qlen * h_jobs[i].tlen, io_bytes += (uint64_t)h_jobs[i].qlen + h_jobs[i].tlen + 40;
 			continue;

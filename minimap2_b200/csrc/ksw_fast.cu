@@ -694,9 +694,8 @@ void mmb_ksw_fast_plan(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, const std::vec
 	A.long_thres = lt, A.long_diff = lt * (e - e2) - (q2 - q) - e2;
 	// The packed kernel needs every intermediate of the recurrence inside [-128, 127] with room to spare, and the simple
 	// match/mismatch scoring; anything else runs the scalar kernel.
-	static const bool no_pk = getenv("MM_B200_NO_PK_KSW") != nullptr;
 	const int amax = std::max(std::abs((int)A.mch), std::max(std::abs((int)A.mis), std::abs((int)A.scn)));
-	const bool pk_ok = !no_pk && 2 * std::max(q + e, q2 + e2) + amax + 8 <= 127 && A.mch > 0 && A.mis <= 0 && A.scn <= 0;
+	const bool pk_ok = 2 * std::max(q + e, q2 + e2) + amax + 8 <= 127 && A.mch > 0 && A.mis <= 0 && A.scn <= 0;
 	// column strips: the smallest C with 32*C >= tlen keeps the idle-lane fraction low (C is a template parameter)
 	static const int CW[] = { 2, 4, 6, 7, 8, 9, 10, 12, 14, 16,   4, 8, 12, 16, 20, 24,   14, 16 };
 	static const int CPW[] = { 4, 4, 8, 8, 8, 16, 16, 16, 16, 16,   4, 8, 16, 16, 32, 32,   16, 16 };

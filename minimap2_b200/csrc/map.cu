@@ -283,48 +283,94 @@ struct MapPass {
 	uint8_t *no_chain;  // out (optional): 1 for reads that went through chaining and came out with no chain at all
 };
 
-static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *qlens, const char **seqs, const char **names,
-					 int *n_regs_out, mm_reg1_t **regs_out, int *rep_len_out, const mm_mapopt_t *opt, int n_threads, const MapPass &pass)
+namespace {
+
+// MM_B200_TIMING: wall time of each section of a group's batch, taken after a stream synchronise
+struct Lap {
+	mmb_ctx_t *ctx;
+	double t_last;
+	static bool on() { static const bool timing = getenv("MM_B200_TIMING") != nullptr; return timing; }
+	void operator()(const char *what)
+	{
+		if (!on()) return;
+		cudaStreamSynchronize(ctx->stream);
+		const double t = realtime();
+		fprintf(stderr, "[timing g%d] %-28s %.1f ms  @ %.1f - %.1f\n", ctx->group_id, what, 1e3 * (t - t_last), 1e3 * (t_last - g_batch_t0), 1e3 * (t - g_batch_t0));
+		t_last = t;
+	}
+};
+
+// One batch of a group on its way through the stages: what every stage reads, and what one stage hands to the next
+struct Batch {
+	mmb_ctx_t *ctx;
+	BatchBufs &bb;
+	bool gated;                        // device phases take a slot of g_gate
+	const mm_idx_t *mi;
+	const mm_mapopt_t *opt;
+	int n_threads;
+	Lap lap;
+	std::vector<int> live;             // input indices of the reads that go through the pipeline (non-empty, within max_qlen)
+	std::vector<int64_t> off;          // n+1 offsets of the live reads back to back
+	int n = 0;
+	int64_t total_bases = 0;
+	uint8_t *d_seq = nullptr;          // the live reads on the device (nt4), their offsets and lengths
+	int64_t *d_off = nullptr;
+	int32_t *d_qlen = nullptr;
+	SeedArgs S;                        // stage 1 device arrays, up to the sorted anchors
+	int64_t total_mz = 0, total_a = 0;
+	// stage 1 results on the host (in bb.h_misc): per-read offsets into the dense chains (u), their anchors (a) and the kept
+	// seed positions (mini_pos), the three dense arrays, and rep_len
+	int64_t *h_uo = nullptr, *h_vo = nullptr, *h_mo = nullptr;
+	m128 *h_da = nullptr;
+	uint64_t *h_du = nullptr, *h_dm = nullptr;
+	int32_t *h_rep = nullptr;
+	size_t keep_used = 0;              // device CIGAR arenas (bb.cig_keep) handed out so far, counted across the waves of the batch
+	int wave = 0;
+	Batch(mmb_ctx_t *c, BatchBufs &b, bool g, const mm_idx_t *m, const mm_mapopt_t *o, int nt)
+		: ctx(c), bb(b), gated(g), mi(m), opt(o), n_threads(nt), lap{c, realtime()} {}
+};
+
+} // namespace
+
+// Resets the per-read state and the outputs of every read, and lists the reads that are mapped. false: there are none.
+static bool take_reads(Batch &b, int n_reads, const int *qlens, const char **seqs, const char **names, int *n_regs_out, mm_reg1_t **regs_out, int *rep_len_out)
 {
-	if (n_reads <= 0) return 0;
-	static const bool timing = getenv("MM_B200_TIMING") != nullptr;
-	double t_last = realtime();
-	auto lap = [&](const char *what) { if (timing) { cudaStreamSynchronize(G.ctx->stream); double t = realtime(); fprintf(stderr, "[timing g%d] %-28s %.1f ms  @ %.1f - %.1f\n", G.ctx->group_id, what, 1e3 * (t - t_last), 1e3 * (t_last - g_batch_t0), 1e3 * (t - g_batch_t0)); t_last = t; } };
-	mm_idx_bucket_s *B = mi->B;
-	mmb_ctx_t *ctx = G.ctx;
-	MMB_CUDA_CHECK(cudaSetDevice(ctx->device));
-	// annotated introns of the index (mm_idx_bed_read) for the spliced kernel: what mm_get_junc / mm_idx_bed_junc feed ksw_exts2 (align.c:638-643)
-	ctx->n_junc = B->n_junc, ctx->junc_st = B->d_junc, ctx->junc_en = B->d_junc? B->d_junc + B->n_junc : nullptr;
-	ctx->junc_strand = B->d_junc? (const int8_t*)(B->d_junc + 2 * B->n_junc) : nullptr;
-	for (int t = 0; t < 2; ++t) // splice scores (mm_idx_spsc_read): what mm_idx_spsc_get feeds ksw_exts2 (align.c:640)
-		ctx->n_spsc[t] = B->n_spsc[t], ctx->spsc_pos[t] = (const int64_t*)B->d_spsc[t], ctx->spsc_val[t] = B->d_spsc[t]? B->d_spsc[t] + B->n_spsc[t] * 8 : nullptr;
-	BatchBufs &bb = G.bb;
-	if (n_threads < 1) n_threads = 1;
+	BatchBufs &bb = b.bb;
 	if ((int)bb.rs_pool.size() < n_reads) bb.rs_pool.resize(n_reads), bb.ra_pool.resize(n_reads);
 	std::vector<ReadState> &rs = bb.rs_pool;
-	std::vector<int64_t> off(n_reads + 1, 0);
-	std::vector<int> live; // reads that go through the pipeline (non-empty, within max_qlen)
 	for (int i = 0; i < n_reads; ++i) {
 		rs[i].qlen = qlens[i], rs[i].seq = seqs[i], rs[i].name = names? names[i] : nullptr;
 		rs[i].ra = nullptr, rs[i].regs0 = nullptr, rs[i].regs = nullptr, rs[i].n_regs = rs[i].n_regs0 = 0, rs[i].done = false, rs[i].fin_pending = false;
 		n_regs_out[i] = 0, regs_out[i] = nullptr;
 		if (rep_len_out) rep_len_out[i] = 0;
-		bool ok = qlens[i] > 0 && !(opt->max_qlen > 0 && qlens[i] > opt->max_qlen); // map.c:243-244
-		if (ok) live.push_back(i);
+		bool ok = qlens[i] > 0 && !(b.opt->max_qlen > 0 && qlens[i] > b.opt->max_qlen); // map.c:243-244
+		if (ok) b.live.push_back(i);
 	}
-	const int n = (int)live.size();
-	if (n == 0) return 0;
-	for (int j = 0; j < n; ++j) off[j + 1] = off[j] + rs[live[j]].qlen;
-	const int64_t total_bases = off[n];
+	const int n = b.n = (int)b.live.size();
+	if (n == 0) return false;
+	b.off.assign((size_t)n + 1, 0);
+	for (int j = 0; j < n; ++j) b.off[j + 1] = b.off[j] + rs[b.live[j]].qlen;
+	b.total_bases = b.off[n];
+	return true;
+}
 
-	lap("setup");
-	// ---------------- stage 1: device ----------------
+// The reads to the device: host concat, H2D and nt4 encoding, the latter two skipped when the reads are resident (the group's
+// previous batch was the same reads). Returns the concatenated reads on the host (ASCII).
+static const uint8_t *upload_reads(GroupCtx &G, Batch &b)
+{
+	mmb_ctx_t *ctx = b.ctx;
+	BatchBufs &bb = b.bb;
+	const std::vector<ReadState> &rs = bb.rs_pool;
+	const std::vector<int> &live = b.live;
+	const std::vector<int64_t> &off = b.off;
+	const int n = b.n;
+	const int64_t total_bases = b.total_bases;
 	uint8_t *h_seq = bb.h_seq.as<uint8_t>((size_t)total_bases + 16);
-	parallel_for(n, n_threads, [&](int64_t j, int) { memcpy(h_seq + off[j], rs[live[j]].seq, rs[live[j]].qlen); });
-	lap("host concat");
-	uint8_t *d_seq = bb.seq.as<uint8_t>((size_t)total_bases + 16);
-	int64_t *d_off = bb.off.as<int64_t>((size_t)n + 1);
-	int32_t *d_qlen = bb.qlen.as<int32_t>((size_t)n);
+	parallel_for(n, b.n_threads, [&](int64_t j, int) { memcpy(h_seq + off[j], rs[live[j]].seq, rs[live[j]].qlen); });
+	b.lap("host concat");
+	uint8_t *d_seq = b.d_seq = bb.seq.as<uint8_t>((size_t)total_bases + 16);
+	int64_t *d_off = b.d_off = bb.off.as<int64_t>((size_t)n + 1);
+	int32_t *d_qlen = b.d_qlen = bb.qlen.as<int32_t>((size_t)n);
 	std::vector<int32_t> h_qlen(n);
 	for (int j = 0; j < n; ++j) h_qlen[j] = rs[live[j]].qlen;
 	const bool resident_hit = mmb_resident_reads() && G.res_n == n && G.res_bases == total_bases && G.res_first == rs[live[0]].seq;
@@ -340,18 +386,30 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 		++ctx->n_launch;
 	}
 	G.res_n = n, G.res_bases = total_bases, G.res_first = rs[live[0]].seq;
-	// the reads are on their way before the group queues for a device slot: every group's upload starts when the batch starts and
-	// overlaps the kernels of the groups ahead of it
-	GateHold gate1(G.gated, 0);
-	lap("gate wait 1");
+	return h_seq;
+}
+
+// Stage 1 from the reads on the device to the sorted anchors: K1 sketch -> query-side filter -> index lookup -> streak selection ->
+// anchor expansion -> anchor sort (collect_minimizers + mm_collect_matches + collect_seed_hits, map.c:59-100,168-204), on the
+// context's stream. Fills b.S, b.total_mz and b.total_a. occ_cut: the max_occ of mm_collect_matches. The optional host work runs
+// between the sketch and the seed selection: SDUST intervals (b.opt->sdust_thres > 0) from h_seq, the reads on the host (ASCII);
+// and skip_seed's query-name bounds when names (by input index) is not null.
+static void seed_batch(Batch &b, const uint8_t *h_seq, const char **names, int occ_cut)
+{
+	mmb_ctx_t *ctx = b.ctx;
+	BatchBufs &bb = b.bb;
+	const mm_idx_t *mi = b.mi;
+	const mm_mapopt_t *opt = b.opt;
+	mm_idx_bucket_s *B = mi->B;
+	const int n = b.n;
 	int64_t *d_mz_off = bb.mz_off.as<int64_t>((size_t)n + 1);
-	const int64_t total_mz = mmb_sketch_device(ctx, d_seq, nullptr, d_off, n, nullptr, 0, mi->w, mi->k, mi->flag & MM_I_HPC, total_bases,
-											   bb.mz, d_mz_off, bb.t1, bb.t2, 1 /* rid = segment index 0 for every read (map.c:65) */);
-	SeedArgs S;
-	S.ix = B->view(mi), S.n_reads = n, S.mz = (m128*)bb.mz.p, S.mz_off = d_mz_off, S.qlen = d_qlen;
+	const int64_t total_mz = b.total_mz = mmb_sketch_device(ctx, b.d_seq, nullptr, b.d_off, n, nullptr, 0, mi->w, mi->k, mi->flag & MM_I_HPC, b.total_bases,
+															bb.mz, d_mz_off, bb.t1, bb.t2, 1 /* rid = segment index 0 for every read (map.c:65) */);
+	SeedArgs &S = b.S;
+	S.ix = B->view(mi), S.n_reads = n, S.mz = (m128*)bb.mz.p, S.mz_off = d_mz_off, S.qlen = b.d_qlen;
 	S.n_mz = bb.n_mz.as<int32_t>((size_t)n);
 	S.q_occ_max = opt->mid_occ, S.q_occ_frac = opt->q_occ_frac;
-	S.max_occ = pass.occ_cut, S.max_max_occ = opt->max_max_occ, S.occ_dist = opt->occ_dist, S.flag = opt->flag;
+	S.max_occ = occ_cut, S.max_max_occ = opt->max_max_occ, S.occ_dist = opt->occ_dist, S.flag = opt->flag;
 	const size_t nm = (size_t)total_mz + 4;
 	S.s_n = bb.s_n.as<uint32_t>(nm), S.s_off = bb.s_off.as<uint64_t>(nm), S.k_idx = bb.k_idx.as<uint32_t>(nm), S.k_aoff = bb.k_aoff.as<uint32_t>(nm);
 	S.flt = bb.flt.as<uint8_t>(nm), S.mini_pos = bb.mini_pos.as<uint64_t>(nm);
@@ -359,8 +417,9 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 	init_nmz_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_mz_off, n, S.n_mz);
 	++ctx->n_launch;
 	if (opt->sdust_thres > 0) { // map.c:68-69: low-complexity masking of the query minimizers; the intervals come from the host
+		const std::vector<int64_t> &off = b.off;
 		std::vector<std::vector<uint64_t>> regs((size_t)n);
-		parallel_for(n, n_threads, [&](int64_t j, int) { hl_sdust((const uint8_t*)rs[live[j]].seq, rs[live[j]].qlen, opt->sdust_thres, 64, regs[j]); });
+		parallel_for(n, b.n_threads, [&](int64_t j, int) { hl_sdust(h_seq + off[j], (int)(off[j + 1] - off[j]), opt->sdust_thres, 64, regs[j]); });
 		std::vector<int64_t> doff((size_t)n + 1, 0);
 		for (int j = 0; j < n; ++j) doff[j + 1] = doff[j] + (int64_t)regs[j].size();
 		std::vector<uint64_t> flat((size_t)doff[n] + 1);
@@ -390,8 +449,8 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 			}
 			std::vector<uint32_t> qlo(n), qhi(n);
 			const std::vector<uint32_t> &ord = B->name_order;
-			parallel_for(n, n_threads, [&](int64_t j, int) {
-				const char *qn = rs[live[j]].name;
+			parallel_for(n, b.n_threads, [&](int64_t j, int) {
+				const char *qn = names[b.live[j]];
 				if (!qn) { qlo[j] = qhi[j] = 0; return; } // no name: no name test (map.c:81)
 				qlo[j] = (uint32_t)(std::lower_bound(ord.begin(), ord.end(), qn, [&](uint32_t id, const char *q) { return strcmp(mi->seq[id].name, q) < 0; }) - ord.begin());
 				qhi[j] = (uint32_t)(std::upper_bound(ord.begin(), ord.end(), qn, [&](const char *q, uint32_t id) { return strcmp(q, mi->seq[id].name) < 0; }) - ord.begin());
@@ -407,11 +466,24 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 	int64_t *d_a_off = bb.a_off.as<int64_t>((size_t)n + 1);
 	copy_i64_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(S.n_a, n, d_a_off);
 	++ctx->n_launch;
-	const int64_t total_a = mmb_exclusive_scan_i64(ctx, d_a_off, n, true);
+	const int64_t total_a = b.total_a = mmb_exclusive_scan_i64(ctx, d_a_off, n, true);
 	S.a = bb.a.as<m128>((size_t)total_a + 4), S.a_off = d_a_off;
 	S.a_sorted = bb.a2.as<m128>((size_t)total_a + 4);
 	mmb_seed_expand_sort_device(ctx, S, total_mz, total_a, bb.stk);
-	lap("h2d+sketch+seed+sort");
+}
+
+// Stage 1 from the sorted anchors to the host: chaining (map.c:262-281), the long-join rescue (map.c:283-292), dense per-read copies
+// of the chains, their anchors and the kept seed positions, and their D2H copy. Drops gate1, the group's device slot, as soon as the
+// copies are in.
+static void chain_batch(Batch &b, const MapPass &pass, GateHold &gate1)
+{
+	mmb_ctx_t *ctx = b.ctx;
+	BatchBufs &bb = b.bb;
+	const mm_mapopt_t *opt = b.opt;
+	const SeedArgs &S = b.S;
+	const int n = b.n;
+	const int64_t total_a = b.total_a;
+	const int64_t *d_a_off = S.a_off;
 	// chaining parameters (map.c:262-281)
 	mmb_chain_par_t cp;
 	memset(&cp, 0, sizeof(cp));
@@ -423,7 +495,7 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 	} else max_chain_gap_ref = opt->max_gap;
 	cp.max_dist_x = max_chain_gap_ref, cp.max_dist_y = max_chain_gap_qry, cp.bw = opt->bw, cp.max_skip = opt->max_chain_skip;
 	cp.max_iter = opt->max_chain_iter, cp.min_cnt = opt->min_cnt, cp.min_sc = opt->min_chain_score;
-	cp.chn_pen_gap = (float)(opt->chain_gap_scale * 0.01 * mi->k), cp.chn_pen_skip = (float)(opt->chain_skip_scale * 0.01 * mi->k);
+	cp.chn_pen_gap = (float)(opt->chain_gap_scale * 0.01 * b.mi->k), cp.chn_pen_skip = (float)(opt->chain_skip_scale * 0.01 * b.mi->k);
 	cp.is_cdna = (opt->flag & MM_F_SPLICE) != 0, cp.n_seg = 1; // map.c:277 (is_splice selects the cDNA gap model of comput_sc)
 	int32_t *d_n_u = bb.n_u.as<int32_t>((size_t)n), *d_n_v = bb.n_v.as<int32_t>((size_t)n);
 	uint64_t *d_u = bb.u.as<uint64_t>((size_t)total_a + 4);
@@ -442,7 +514,7 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 		const int64_t tv = mmb_exclusive_scan_i64(ctx, d_vo, n, true);
 		RescuePar rp;
 		rp.primary = 0;
-		rp.qlen = d_qlen, rp.rescue_size = opt->rmq_rescue_size, rp.rescue_ratio = opt->rmq_rescue_ratio;
+		rp.qlen = b.d_qlen, rp.rescue_size = opt->rmq_rescue_size, rp.rescue_ratio = opt->rmq_rescue_ratio;
 		rp.max_dist = opt->max_gap, rp.max_dist_inner = opt->rmq_inner_dist, rp.bw = opt->bw_long, rp.max_skip = opt->max_chain_skip;
 		rp.rmq_size_cap = opt->rmq_size_cap, rp.min_cnt = opt->min_cnt, rp.min_sc = opt->min_chain_score;
 		rp.pen_gap = cp.chn_pen_gap, rp.pen_skip = cp.chn_pen_skip, rp.tree = nullptr, rp.tree_off = d_vo;
@@ -461,15 +533,16 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 	const unsigned gw = (unsigned)(((int64_t)n * 32 + 255) / 256);
 	gather_kernel<uint64_t><<<gw, 256, 0, ctx->stream>>>(d_u, d_a_off, d_n_u, d_uo, n, d_du);
 	gather_kernel<m128><<<gw, 256, 0, ctx->stream>>>(d_a_out, d_a_off, d_n_v, d_vo, n, d_da);
-	gather_kernel<uint64_t><<<gw, 256, 0, ctx->stream>>>(S.mini_pos, d_mz_off, S.n_keep, d_mo, n, d_dm);
+	gather_kernel<uint64_t><<<gw, 256, 0, ctx->stream>>>(S.mini_pos, S.mz_off, S.n_keep, d_mo, n, d_dm);
 	ctx->n_launch += 3;
 	// host copies
 	const size_t misc_bytes = sizeof(int64_t) * (size_t)(n + 1) * 3 + sizeof(int32_t) * (size_t)n + sizeof(uint64_t) * (size_t)(tot_u + tot_m) + sizeof(m128) * (size_t)tot_v + 64;
 	uint8_t *hm = bb.h_misc.as<uint8_t>(misc_bytes);
-	int64_t *h_uo = (int64_t*)hm, *h_vo = h_uo + (n + 1), *h_mo = h_vo + (n + 1);
-	m128 *h_da = (m128*)(h_mo + (n + 1));
-	uint64_t *h_du = (uint64_t*)(h_da + tot_v), *h_dm = h_du + tot_u;
-	int32_t *h_rep = (int32_t*)(h_dm + tot_m);
+	int64_t *h_uo = b.h_uo = (int64_t*)hm;
+	b.h_vo = h_uo + (n + 1), b.h_mo = b.h_vo + (n + 1);
+	m128 *h_da = b.h_da = (m128*)(b.h_mo + (n + 1));
+	uint64_t *h_du = b.h_du = (uint64_t*)(h_da + tot_v), *h_dm = b.h_dm = h_du + tot_u;
+	int32_t *h_rep = b.h_rep = (int32_t*)(h_dm + tot_m);
 	MMB_CUDA_CHECK(cudaMemcpyAsync(h_uo, d_doff, sizeof(int64_t) * (size_t)(n + 1) * 3, cudaMemcpyDeviceToHost, ctx->stream));
 	MMB_CUDA_CHECK(cudaMemcpyAsync(h_da, d_da, sizeof(m128) * (size_t)tot_v, cudaMemcpyDeviceToHost, ctx->stream));
 	MMB_CUDA_CHECK(cudaMemcpyAsync(h_du, d_du, sizeof(uint64_t) * (size_t)tot_u, cudaMemcpyDeviceToHost, ctx->stream));
@@ -479,24 +552,35 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 	gate1.drop();
 	ctx->last_d2h_bytes += misc_bytes;
 	if (ctx->profiling) {
-		ctx->prof_bytes[MMB_PROF_SKETCH] += (uint64_t)(total_bases / 4) + 16ull * (uint64_t)total_mz;
+		const int64_t total_mz = b.total_mz;
+		ctx->prof_bytes[MMB_PROF_SKETCH] += (uint64_t)(b.total_bases / 4) + 16ull * (uint64_t)total_mz;
 		ctx->prof_bytes[MMB_PROF_SEED] += 32ull * (uint64_t)total_mz + 24ull * (uint64_t)total_a;
 		ctx->prof_bytes[MMB_PROF_SORT] += 32ull * (uint64_t)total_a;
 		ctx->prof_bytes[MMB_PROF_CHAIN] += 16ull * (uint64_t)total_a + 16ull * (uint64_t)tot_v + 8ull * (uint64_t)tot_u;
 	}
+}
 
-	lap("chain+rescue+d2h");
-	// ---------------- stage 2: chains -> hits (map.c:317-336) ----------------
+// Stage 2 (map.c:317-336): chains -> hits on the host threads. Reads with hits to align (MM_F_CIGAR) get their alignment state;
+// the others are done.
+static void chains_to_hits(Batch &b, const MapPass &pass)
+{
+	BatchBufs &bb = b.bb;
+	std::vector<ReadState> &rs = bb.rs_pool;
+	const std::vector<int> &live = b.live;
+	const std::vector<int64_t> &off = b.off;
+	const mm_idx_t *mi = b.mi;
+	const mm_mapopt_t *opt = b.opt;
+	const int n = b.n;
 	const bool with_cigar = (opt->flag & MM_F_CIGAR) != 0;
-	if (with_cigar && bb.qseq_pool.size() < (size_t)total_bases * 2 + 16) bb.qseq_pool.resize((size_t)total_bases * 2 + 16);
-	parallel_for(n, n_threads, [&](int64_t j, int) {
+	if (with_cigar && bb.qseq_pool.size() < (size_t)b.total_bases * 2 + 16) bb.qseq_pool.resize((size_t)b.total_bases * 2 + 16);
+	parallel_for(n, b.n_threads, [&](int64_t j, int) {
 		HpScope hp_(HP_HITS);
 		ReadState &r = rs[live[j]];
-		r.rep_len = h_rep[j];
-		r.n_u = (int)(h_uo[j + 1] - h_uo[j]), r.u = h_du + h_uo[j];
+		r.rep_len = b.h_rep[j];
+		r.n_u = (int)(b.h_uo[j + 1] - b.h_uo[j]), r.u = b.h_du + b.h_uo[j];
 		if (pass.no_chain) pass.no_chain[live[j]] = r.n_u == 0;
-		r.n_a = (int)(h_vo[j + 1] - h_vo[j]), r.a_src = h_da + h_vo[j];
-		r.n_mini_pos = (int)(h_mo[j + 1] - h_mo[j]), r.mini_pos = h_dm + h_mo[j];
+		r.n_a = (int)(b.h_vo[j + 1] - b.h_vo[j]), r.a_src = b.h_da + b.h_vo[j];
+		r.n_mini_pos = (int)(b.h_mo[j + 1] - b.h_mo[j]), r.mini_pos = b.h_dm + b.h_mo[j];
 		uint32_t hash = r.name && !(opt->flag & MM_F_NO_HASH_NAME)? x31_hash_string(r.name) : 0; // map.c:246-248
 		hash ^= wang_hash((uint32_t)r.qlen) + wang_hash((uint32_t)opt->seed);
 		r.hash = wang_hash(hash);
@@ -524,7 +608,7 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 		} else r.done = true, r.n_regs = n_regs0, r.regs = regs0, r.regs0 = nullptr;
 	});
 
-	lap("stage2 host hits");
+	b.lap("stage2 host hits");
 	if (with_cigar) { // nt4 forward / reverse-complement copies of the reads (align.c:1056-1061): room is set aside, the copies are made on first use
 		for (int j = 0; j < n; ++j) {
 			ReadState &r = rs[live[j]];
@@ -534,264 +618,298 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 			r.ra->qseq[0] = q0, r.ra->qseq[1] = q0 + r.qlen;
 		}
 	}
-	lap("stage2 qseq encode");
-	// ---------------- stage 3: alignment waves ----------------
-	if (with_cigar) {
-		mmb_ksw_score_t sc;
-		{ // align.c:11-38 via a throw-away driver-compatible matrix
-			const int m = 5;
-			int8_t aa = (int8_t)(opt->a < 0? -opt->a : opt->a), bb2 = (int8_t)(opt->b > 0? -opt->b : opt->b);
-			int8_t sa = (int8_t)(opt->sc_ambi > 0? -opt->sc_ambi : opt->sc_ambi);
-			for (int i = 0; i < m - 1; ++i) { for (int k = 0; k < m - 1; ++k) sc.mat[i * m + k] = i == k? aa : bb2; sc.mat[i * m + m - 1] = sa; }
-			for (int k = 0; k < m; ++k) sc.mat[(m - 1) * m + k] = sa;
-			if (!(opt->transition == 0 || opt->transition == opt->b)) {
-				int8_t t = (int8_t)(opt->transition > 0? -opt->transition : opt->transition);
-				sc.mat[0 * m + 2] = t, sc.mat[1 * m + 3] = t, sc.mat[2 * m + 0] = t, sc.mat[3 * m + 1] = t;
-			}
-			sc.q = (int8_t)opt->q, sc.e = (int8_t)opt->e, sc.q2 = (int8_t)opt->q2, sc.e2 = (int8_t)opt->e2;
-			sc.noncan = (int8_t)opt->noncan, sc.junc_bonus = (int8_t)opt->junc_bonus, sc.junc_pen = (int8_t)opt->junc_pen;
-			// mm_test_zdrop only compares the largest drop with zdrop and (unless the inversion probe is off, align.c:92) zdrop_inv: a
-			// path whose total penalty stays below both needs no scan
-			{
-				const bool inv_off = (opt->flag & (MM_F_SPLICE | MM_F_SR | MM_F_FOR_ONLY | MM_F_REV_ONLY)) != 0;
-				const int th = inv_off? opt->zdrop : std::min(opt->zdrop, opt->zdrop_inv);
-				sc.zd_skip = (int16_t)std::max(0, std::min(th, 30000));
-			}
+	b.lap("stage2 qseq encode");
+}
+
+// the ksw2 scoring of the options: align.c:11-38 via a throw-away driver-compatible matrix
+static mmb_ksw_score_t ksw_score(const mm_mapopt_t *opt)
+{
+	mmb_ksw_score_t sc;
+	const int m = 5;
+	int8_t aa = (int8_t)(opt->a < 0? -opt->a : opt->a), bb2 = (int8_t)(opt->b > 0? -opt->b : opt->b);
+	int8_t sa = (int8_t)(opt->sc_ambi > 0? -opt->sc_ambi : opt->sc_ambi);
+	for (int i = 0; i < m - 1; ++i) { for (int k = 0; k < m - 1; ++k) sc.mat[i * m + k] = i == k? aa : bb2; sc.mat[i * m + m - 1] = sa; }
+	for (int k = 0; k < m; ++k) sc.mat[(m - 1) * m + k] = sa;
+	if (!(opt->transition == 0 || opt->transition == opt->b)) {
+		int8_t t = (int8_t)(opt->transition > 0? -opt->transition : opt->transition);
+		sc.mat[0 * m + 2] = t, sc.mat[1 * m + 3] = t, sc.mat[2 * m + 0] = t, sc.mat[3 * m + 1] = t;
+	}
+	sc.q = (int8_t)opt->q, sc.e = (int8_t)opt->e, sc.q2 = (int8_t)opt->q2, sc.e2 = (int8_t)opt->e2;
+	sc.noncan = (int8_t)opt->noncan, sc.junc_bonus = (int8_t)opt->junc_bonus, sc.junc_pen = (int8_t)opt->junc_pen;
+	// mm_test_zdrop only compares the largest drop with zdrop and (unless the inversion probe is off, align.c:92) zdrop_inv: a
+	// path whose total penalty stays below both needs no scan
+	const bool inv_off = (opt->flag & (MM_F_SPLICE | MM_F_SR | MM_F_FOR_ONLY | MM_F_REV_ONLY)) != 0;
+	const int th = inv_off? opt->zdrop : std::min(opt->zdrop, opt->zdrop_inv);
+	sc.zd_skip = (int16_t)std::max(0, std::min(th, 30000));
+	return sc;
+}
+
+// align_regs (map.c:215-225): the read's aligned hits get their parents and secondaries; the read is done
+static void post_align(const Batch &b, ReadState &r, int n_regs, mm_reg1_t *regs)
+{
+	HpScope hp_(HP_POST);
+	const mm_mapopt_t *opt = b.opt;
+	if (!(opt->flag & MM_F_ALL_CHAINS)) {
+		hl_set_parent(opt->mask_level, opt->mask_len, n_regs, regs, opt->a * 2 + opt->b, opt->flag & MM_F_HARD_MLEVEL, opt->alt_drop);
+		hl_select_sub(opt->pri_ratio, b.mi->k * 2, opt->best_n, 0, (int)(opt->max_gap * 0.8), &n_regs, regs);
+		hl_set_sam_pri(n_regs, regs);
+	}
+	r.n_regs = n_regs, r.regs = regs, r.done = true, r.fin_pending = false;
+}
+
+// one pass of the alignment driver over the read's pristine chains
+static mm_reg1_t *replay_read(const Batch &b, ReadState &r, bool defer, int *n_regs_out)
+{
+	ReadAlign &ra = *r.ra;
+	int n_regs = r.n_regs0;
+	mm_reg1_t *regs;
+	{
+		HpScope hp_(HP_PRE);
+		r.a.assign(r.a_src, r.a_src + r.n_a); // pristine anchors (IGNORE/LONG_JOIN marks cleared)
+		regs = (mm_reg1_t*)malloc(sizeof(mm_reg1_t) * (n_regs > 0? n_regs : 1));
+		memcpy(regs, r.regs0, sizeof(mm_reg1_t) * n_regs);
+	}
+	ra.defer = defer;
+	regs = hl_align_skeleton(b.opt, b.mi, ra, &n_regs, regs, r.n_a, r.a.data());
+	*n_regs_out = n_regs;
+	return regs;
+}
+
+static void drop_regs(int n_regs, mm_reg1_t *regs) { for (int i = 0; i < n_regs; ++i) free(regs[i].p); free(regs); }
+
+// K4: the device tail (CIGAR assembly, mm_fix_cigar, mm_update_extra) for the reads of the wave whose replay is complete
+static void device_tail(Batch &b, const std::vector<int> &active, const FinPar &fpar)
+{
+	std::vector<ReadState> &rs = b.bb.rs_pool;
+	std::vector<int> fr;
+	for (size_t t = 0; t < active.size(); ++t) if (rs[active[t]].fin_pending) fr.push_back(active[t]);
+	if (fr.empty()) return;
+	mmb_ctx_t *ctx = b.ctx;
+	BatchBufs &bb = b.bb;
+	const mm_idx_t *mi = b.mi;
+	const size_t nf = fr.size();
+	std::vector<int64_t> hoff(nf + 1, 0), joff2(nf + 1, 0);
+	for (size_t t = 0; t < nf; ++t) {
+		const ReadAlign &ra = *rs[fr[t]].ra;
+		hoff[t + 1] = hoff[t] + (int64_t)ra.fin_hits.size(), joff2[t + 1] = joff2[t] + (int64_t)ra.fin_jobs.size();
+	}
+	const int64_t n_hits = hoff[nf], n_pieces = joff2[nf];
+	std::vector<int64_t> coff((size_t)n_hits + 1, 0); // output CIGAR offsets (room for the sum of the pieces)
+	for (size_t t = 0; t < nf; ++t) {
+		const ReadAlign &ra = *rs[fr[t]].ra;
+		for (size_t k = 0; k < ra.fin_hits.size(); ++k) coff[hoff[t] + k + 1] = ra.fin_hits[k].n_cig_max;
+	}
+	for (int64_t i = 0; i < n_hits; ++i) coff[i + 1] += coff[i];
+	const int64_t tot_cig = coff[n_hits];
+	const size_t in_bytes = sizeof(FinReg) * (size_t)n_hits + sizeof(FinJobRef) * (size_t)n_pieces;
+	uint8_t *h_in = bb.h_fin_in.as<uint8_t>(in_bytes + 64);
+	FinReg *h_regs = (FinReg*)h_in;
+	FinJobRef *h_pieces = (FinJobRef*)(h_regs + n_hits);
+	parallel_for((int64_t)nf, b.n_threads, [&](int64_t t, int) {
+		const ReadState &r = rs[fr[t]];
+		const ReadAlign &ra = *r.ra;
+		for (size_t k = 0; k < ra.fin_jobs.size(); ++k) { FinJobRef &j = h_pieces[joff2[t] + k]; j.cig = ra.fin_jobs[k].dcig, j.n = ra.fin_jobs[k].n, j.pad = 0; }
+		for (size_t k = 0; k < ra.fin_hits.size(); ++k) {
+			const HlFinHit &h = ra.fin_hits[k];
+			FinReg &f = h_regs[hoff[t] + k];
+			f.q0 = ra.q_dev_off, f.t0 = (int64_t)mi->seq[h.rid].offset + h.rs, f.out_off = coff[hoff[t] + k];
+			f.qlen = r.qlen, f.qs = h.qs, f.rev = h.rev, f.qspan = h.qspan, f.tspan = h.tspan;
+			f.job_first = (int32_t)(joff2[t] + h.job_first), f.n_jobs = h.n_jobs, f.pad = 0;
 		}
-		std::vector<int> active;
-		for (int j = 0; j < n; ++j) if (!rs[live[j]].done) active.push_back(live[j]);
-		// The hit-level tail of the driver (CIGAR assembly, mm_fix_cigar, mm_update_extra) runs on the device for finished reads (K4,
-		// finalize.cu) unless the mode needs it on the host (spliced / =X CIGARs / query-strand) or MM_B200_NO_DEV_FIN is set.
-		static const bool no_dev_fin = getenv("MM_B200_NO_DEV_FIN") != nullptr;
-		const bool use_fin = !no_dev_fin && hl_defer_supported(opt);
-		FinPar fpar;
-		for (int i = 0; i < 25; ++i) fpar.mat[i] = sc.mat[i];
-		fpar.q = (int8_t)opt->q, fpar.e = (int8_t)opt->e, fpar.log_gap = 1;
-		auto post_align = [&](ReadState &r, int n_regs, mm_reg1_t *regs) { // align_regs (map.c:215-225)
-			HpScope hp_(HP_POST);
-			if (!(opt->flag & MM_F_ALL_CHAINS)) {
-				hl_set_parent(opt->mask_level, opt->mask_len, n_regs, regs, opt->a * 2 + opt->b, opt->flag & MM_F_HARD_MLEVEL, opt->alt_drop);
-				hl_select_sub(opt->pri_ratio, mi->k * 2, opt->best_n, 0, (int)(opt->max_gap * 0.8), &n_regs, regs);
-				hl_set_sam_pri(n_regs, regs);
+	});
+	uint8_t *d_in = bb.fin_in.as<uint8_t>(in_bytes + 64);
+	const size_t out_bytes = sizeof(FinOut) * (size_t)n_hits + 4 * (size_t)tot_cig;
+	uint8_t *d_out = bb.fin_out.as<uint8_t>(out_bytes + 64);
+	uint8_t *h_out = bb.h_fin_out.as<uint8_t>(out_bytes + 64);
+	MMB_CUDA_CHECK(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+	mmb_finalize_device(ctx, (const FinReg*)d_in, (const FinJobRef*)(d_in + sizeof(FinReg) * (size_t)n_hits), (int)n_hits, b.d_seq, (const uint32_t*)mi->B->d_S,
+						(uint32_t*)(d_out + sizeof(FinOut) * (size_t)n_hits), (FinOut*)d_out, fpar);
+	MMB_CUDA_CHECK(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+	MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+	ctx->last_h2d_bytes += in_bytes, ctx->last_d2h_bytes += out_bytes;
+	b.lap("  device tail");
+	const HlFinOut *h_fin = (const HlFinOut*)h_out;
+	const uint32_t *h_fcig = (const uint32_t*)(h_out + sizeof(FinOut) * (size_t)n_hits);
+	parallel_for((int64_t)nf, b.n_threads, [&](int64_t t, int) {
+		hl_hp_flush();
+		ReadState &r = rs[fr[t]];
+		ReadAlign &ra = *r.ra;
+		std::vector<const uint32_t*> cp(ra.fin_hits.size());
+		for (size_t k = 0; k < cp.size(); ++k) cp[k] = h_fcig + coff[hoff[t] + k];
+		int n_regs = r.n_regs;
+		mm_reg1_t *regs = r.regs;
+		bool ok;
+		{ HpScope hp_(HP_EXTRA); ok = hl_align_apply_fin(ra, n_regs, regs, h_fin + hoff[t], cp.data()); }
+		if (ok) hl_align_finish(b.opt, ra, &n_regs, regs);
+		else { // a gap penalty outside the fixed-point range (never with sane scoring): the host driver redoes the read
+			drop_regs(n_regs, regs);
+			regs = replay_read(b, r, false, &n_regs);
+			if (ra.incomplete) { fprintf(stderr, "[ERROR] minimap2_b200: host redo of a finished read is incomplete\n"); abort(); }
+		}
+		post_align(b, r, n_regs, regs);
+	});
+	b.lap("  tail apply");
+}
+
+// One K3 wave: the ksw2 jobs the unfinished reads of the wave asked for run in chunks on the device, and the results are handed to
+// the per-read caches. Returns the number of jobs.
+static int64_t ksw_wave(Batch &b, const std::vector<int> &active, const mmb_ksw_score_t &sc)
+{
+	mmb_ctx_t *ctx = b.ctx;
+	BatchBufs &bb = b.bb;
+	std::vector<ReadState> &rs = bb.rs_pool;
+	// gather jobs
+	std::vector<int64_t> joff(active.size() + 1, 0);
+	for (size_t t = 0; t < active.size(); ++t) {
+		ReadState &r = rs[active[t]];
+		joff[t + 1] = joff[t] + (r.done? 0 : (int64_t)r.ra->want.size());
+	}
+	const int64_t n_jobs = joff[active.size()];
+	if (n_jobs == 0) return 0;
+	// every wave executes all jobs the replays asked for, so each read advances by at least one ksw call per wave and the
+	// loop ends; reads that keep splitting under a very small z-drop (-z 30) legitimately need dozens of waves. The
+	// bound only guards against a logic error.
+	if (b.wave >= 100000) { fprintf(stderr, "[ERROR] minimap2_b200: too many alignment waves\n"); abort(); }
+	mmb_ksw_job_t *jobs = bb.h_jobs.as<mmb_ksw_job_t>((size_t)n_jobs);
+	parallel_for((int64_t)active.size(), b.n_threads, [&](int64_t t, int) {
+		ReadState &r = rs[active[t]];
+		if (!r.done && !r.ra->want.empty()) memcpy(&jobs[joff[t]], r.ra->want.data(), sizeof(mmb_ksw_job_t) * r.ra->want.size());
+	});
+	// run in chunks to bound the device result buffers; results land in pinned host memory that stays alive until
+	// the end of the batch, so per-read caches just point into it
+	static const int64_t CH = getenv("MM_B200_JOB_CHUNK")? std::max(1, atoi(getenv("MM_B200_JOB_CHUNK"))) : 1 << 20; // test hook: tiny chunks exercise the multi-chunk bookkeeping
+	mmb_ksw_res_t *res = bb.h_res.as<mmb_ksw_res_t>((size_t)n_jobs);
+	// CIGAR arena estimate per job: (qlen+tlen)/2 + 8 operations covers every realistic alignment, the true bound is qlen+tlen
+	// (alternating 1I1D); an overflow is recovered below by rerunning the chunk with the exact size the kernels reported
+	// and growing the host staging buffer. MM_B200_CIG_SHIFT (test hook) shrinks the estimate to force that path.
+	static const int cig_shift = getenv("MM_B200_CIG_SHIFT")? atoi(getenv("MM_B200_CIG_SHIFT")) : 0;
+	// (a spliced job's target spans its introns, each a single N operation: only a query-sized part of the target can turn into operations)
+	auto cig_est = [&](const mmb_ksw_job_t &jb) -> int64_t {
+		if (jb.flag & MMB_JOB_LL) return 0;
+		const int64_t t_eff = (jb.flag & MMB_JOB_SPLICE)? std::min<int64_t>(jb.tlen, 2 * (int64_t)jb.qlen + 64) : jb.tlen;
+		return (((int64_t)jb.qlen + t_eff) / 2 + 8 >> cig_shift) + 1;
+	};
+	// with the device tail on, every (wave, chunk) keeps its arena until the batch ends (K4 reads the pieces in place);
+	// otherwise one arena is reused, as the host has its copy (spliced jobs reserve room for intron-sized CIGAR estimates)
+	const bool keep_arenas = hl_defer_supported(b.opt);
+	int64_t cap_tot = 0;
+	for (int64_t i = 0; i < n_jobs; ++i) cap_tot += cig_est(jobs[i]);
+	while (bb.h_cig.size() <= (size_t)b.wave) bb.h_cig.emplace_back(new PinBuf);
+	uint32_t *h_cig = bb.h_cig[b.wave]->as<uint32_t>((size_t)cap_tot + 64);
+	GateHold gatew(b.gated, 1);
+	b.lap("  gate wait w");
+	std::vector<int64_t> chunk_base; // offset of each chunk's CIGAR block inside h_cig
+	std::vector<const uint32_t*> chunk_dev; // and the block's address in its device arena
+	int64_t cig_fill = 0;
+	for (int64_t c0 = 0; c0 < n_jobs; c0 += CH) {
+		const int64_t m = std::min(CH, n_jobs - c0);
+		int64_t cap = 0;
+		for (int64_t i = 0; i < m; ++i) cap += cig_est(jobs[c0 + i]);
+		for (;;) {
+			mmb_ksw_job_t *d_jobs = bb.jobs.as<mmb_ksw_job_t>((size_t)m);
+			mmb_ksw_res_t *d_res = bb.res.as<mmb_ksw_res_t>((size_t)m);
+			const size_t ki = keep_arenas? b.keep_used : 0;
+			while (bb.cig_keep.size() <= ki) bb.cig_keep.emplace_back(new DevBuf);
+			uint32_t *d_cig = bb.cig_keep[ki]->as<uint32_t>((size_t)cap + 4);
+			unsigned long long *d_used = (unsigned long long*)d_cig;
+			MMB_CUDA_CHECK(cudaMemcpyAsync(d_jobs, &jobs[c0], sizeof(mmb_ksw_job_t) * m, cudaMemcpyHostToDevice, ctx->stream));
+			MMB_CUDA_CHECK(cudaMemsetAsync(d_used, 0, 8, ctx->stream));
+			mmb_ksw_launch(ctx, &sc, (int)m, &jobs[c0], d_jobs, b.d_seq, b.mi->B->d_S, 1, d_res, d_cig + 2, cap, d_used);
+			unsigned long long used = 0;
+			MMB_CUDA_CHECK(cudaMemcpyAsync(&res[c0], d_res, sizeof(mmb_ksw_res_t) * m, cudaMemcpyDeviceToHost, ctx->stream));
+			MMB_CUDA_CHECK(cudaMemcpyAsync(&used, d_used, 8, cudaMemcpyDeviceToHost, ctx->stream));
+			MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+			if ((int64_t)used > cap) { cap = (int64_t)used + 16; continue; } // rare: rerun the chunk with a larger CIGAR arena
+			if (cig_fill + (int64_t)used > cap_tot) { // grow the wave's host staging buffer, keeping the chunks already staged
+				int64_t rest = 0;
+				for (int64_t i = c0 + m; i < n_jobs; ++i) rest += cig_est(jobs[i]);
+				const int64_t new_tot = cig_fill + (int64_t)used + rest + 64;
+				std::unique_ptr<PinBuf> nb(new PinBuf);
+				uint32_t *np_ = nb->as<uint32_t>((size_t)new_tot + 64);
+				if (cig_fill) memcpy(np_, h_cig, (size_t)cig_fill * 4);
+				bb.h_cig[b.wave]->release();
+				bb.h_cig[b.wave] = std::move(nb);
+				h_cig = np_, cap_tot = new_tot;
 			}
-			r.n_regs = n_regs, r.regs = regs, r.done = true, r.fin_pending = false;
-		};
-		auto replay = [&](ReadState &r, bool defer, int *n_regs_out_) -> mm_reg1_t* { // one pass of the driver over the read's pristine chains
-			ReadAlign &ra = *r.ra;
-			int n_regs = r.n_regs0;
-			mm_reg1_t *regs;
-			{
-				HpScope hp_(HP_PRE);
-				r.a.assign(r.a_src, r.a_src + r.n_a); // pristine anchors (IGNORE/LONG_JOIN marks cleared)
-				regs = (mm_reg1_t*)malloc(sizeof(mm_reg1_t) * (n_regs > 0? n_regs : 1));
-				memcpy(regs, r.regs0, sizeof(mm_reg1_t) * n_regs);
-			}
-			ra.defer = defer;
-			regs = hl_align_skeleton(opt, mi, ra, &n_regs, regs, r.n_a, r.a.data());
-			*n_regs_out_ = n_regs;
-			return regs;
-		};
-		auto drop_regs = [](int n_regs, mm_reg1_t *regs) { for (int i = 0; i < n_regs; ++i) free(regs[i].p); free(regs); };
-		size_t keep_used = 0;
-		int wave = 0;
-		while (!active.empty()) {
-			// replay every active read; collect the jobs they miss
-			parallel_for((int64_t)active.size(), n_threads, [&](int64_t t, int) {
-				hl_hp_flush();
-				ReadState &r = rs[active[t]];
-				ReadAlign &ra = *r.ra;
-				ra.want.clear(); ra.want_slot.clear();
-				int n_regs;
-				mm_reg1_t *regs = replay(r, use_fin, &n_regs);
-				if (ra.defer_abort) { // an inversion probe needs final hit coordinates: this read keeps the whole driver on the host
-					drop_regs(n_regs, regs);
-					regs = replay(r, false, &n_regs); // jobs the aborted pass asked for stay queued (the full pass asks for a superset)
-				}
-				if (ra.incomplete) drop_regs(n_regs, regs);
-				else if (ra.defer && !ra.fin_hits.empty()) r.n_regs = n_regs, r.regs = regs, r.fin_pending = true;
-				else post_align(r, n_regs, regs);
-			});
-			lap("  wave replay");
-			// ---- K4: device tail for the reads whose replay is complete ----
-			{
-				std::vector<int> fr;
-				for (size_t t = 0; t < active.size(); ++t) if (rs[active[t]].fin_pending) fr.push_back(active[t]);
-				if (!fr.empty()) {
-					const size_t nf = fr.size();
-					std::vector<int64_t> hoff(nf + 1, 0), joff2(nf + 1, 0);
-					for (size_t t = 0; t < nf; ++t) {
-						const ReadAlign &ra = *rs[fr[t]].ra;
-						hoff[t + 1] = hoff[t] + (int64_t)ra.fin_hits.size(), joff2[t + 1] = joff2[t] + (int64_t)ra.fin_jobs.size();
-					}
-					const int64_t n_hits = hoff[nf], n_pieces = joff2[nf];
-					std::vector<int64_t> coff((size_t)n_hits + 1, 0); // output CIGAR offsets (room for the sum of the pieces)
-					for (size_t t = 0; t < nf; ++t) {
-						const ReadAlign &ra = *rs[fr[t]].ra;
-						for (size_t k = 0; k < ra.fin_hits.size(); ++k) coff[hoff[t] + k + 1] = ra.fin_hits[k].n_cig_max;
-					}
-					for (int64_t i = 0; i < n_hits; ++i) coff[i + 1] += coff[i];
-					const int64_t tot_cig = coff[n_hits];
-					const size_t in_bytes = sizeof(FinReg) * (size_t)n_hits + sizeof(FinJobRef) * (size_t)n_pieces;
-					uint8_t *h_in = bb.h_fin_in.as<uint8_t>(in_bytes + 64);
-					FinReg *h_regs = (FinReg*)h_in;
-					FinJobRef *h_pieces = (FinJobRef*)(h_regs + n_hits);
-					parallel_for((int64_t)nf, n_threads, [&](int64_t t, int) {
-						const ReadState &r = rs[fr[t]];
-						const ReadAlign &ra = *r.ra;
-						for (size_t k = 0; k < ra.fin_jobs.size(); ++k) { FinJobRef &j = h_pieces[joff2[t] + k]; j.cig = ra.fin_jobs[k].dcig, j.n = ra.fin_jobs[k].n, j.pad = 0; }
-						for (size_t k = 0; k < ra.fin_hits.size(); ++k) {
-							const HlFinHit &h = ra.fin_hits[k];
-							FinReg &f = h_regs[hoff[t] + k];
-							f.q0 = ra.q_dev_off, f.t0 = (int64_t)mi->seq[h.rid].offset + h.rs, f.out_off = coff[hoff[t] + k];
-							f.qlen = r.qlen, f.qs = h.qs, f.rev = h.rev, f.qspan = h.qspan, f.tspan = h.tspan;
-							f.job_first = (int32_t)(joff2[t] + h.job_first), f.n_jobs = h.n_jobs, f.pad = 0;
-						}
-					});
-					uint8_t *d_in = bb.fin_in.as<uint8_t>(in_bytes + 64);
-					const size_t out_bytes = sizeof(FinOut) * (size_t)n_hits + 4 * (size_t)tot_cig;
-					uint8_t *d_out = bb.fin_out.as<uint8_t>(out_bytes + 64);
-					uint8_t *h_out = bb.h_fin_out.as<uint8_t>(out_bytes + 64);
-					MMB_CUDA_CHECK(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
-					mmb_finalize_device(ctx, (const FinReg*)d_in, (const FinJobRef*)(d_in + sizeof(FinReg) * (size_t)n_hits), (int)n_hits, d_seq, (const uint32_t*)B->d_S,
-										(uint32_t*)(d_out + sizeof(FinOut) * (size_t)n_hits), (FinOut*)d_out, fpar);
-					MMB_CUDA_CHECK(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-					MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-					ctx->last_h2d_bytes += in_bytes, ctx->last_d2h_bytes += out_bytes;
-					lap("  device tail");
-					const HlFinOut *h_fin = (const HlFinOut*)h_out;
-					const uint32_t *h_fcig = (const uint32_t*)(h_out + sizeof(FinOut) * (size_t)n_hits);
-					parallel_for((int64_t)nf, n_threads, [&](int64_t t, int) {
-						hl_hp_flush();
-						ReadState &r = rs[fr[t]];
-						ReadAlign &ra = *r.ra;
-						std::vector<const uint32_t*> cp(ra.fin_hits.size());
-						for (size_t k = 0; k < cp.size(); ++k) cp[k] = h_fcig + coff[hoff[t] + k];
-						int n_regs = r.n_regs;
-						mm_reg1_t *regs = r.regs;
-						bool ok;
-						{ HpScope hp_(HP_EXTRA); ok = hl_align_apply_fin(ra, n_regs, regs, h_fin + hoff[t], cp.data()); }
-						if (ok) hl_align_finish(opt, ra, &n_regs, regs);
-						else { // a gap penalty outside the fixed-point range (never with sane scoring): the host driver redoes the read
-							drop_regs(n_regs, regs);
-							regs = replay(r, false, &n_regs);
-							if (ra.incomplete) { fprintf(stderr, "[ERROR] minimap2_b200: host redo of a finished read is incomplete\n"); abort(); }
-						}
-						post_align(r, n_regs, regs);
-					});
-					lap("  tail apply");
-				}
-			}
-			// gather jobs
-			std::vector<int> still;
-			std::vector<int64_t> joff(active.size() + 1, 0);
-			for (size_t t = 0; t < active.size(); ++t) {
-				ReadState &r = rs[active[t]];
-				joff[t + 1] = joff[t] + (r.done? 0 : (int64_t)r.ra->want.size());
-			}
-			const int64_t n_jobs = joff[active.size()];
-			if (n_jobs > 0) {
-				// every wave executes all jobs the replays asked for, so each read advances by at least one ksw call per wave and the
-				// loop ends; reads that keep splitting under a very small z-drop (-z 30) legitimately need dozens of waves. The
-				// bound only guards against a logic error.
-				if (wave >= 100000) { fprintf(stderr, "[ERROR] minimap2_b200: too many alignment waves\n"); abort(); }
-				mmb_ksw_job_t *jobs = bb.h_jobs.as<mmb_ksw_job_t>((size_t)n_jobs);
-				parallel_for((int64_t)active.size(), n_threads, [&](int64_t t, int) {
-					ReadState &r = rs[active[t]];
-					if (!r.done && !r.ra->want.empty()) memcpy(&jobs[joff[t]], r.ra->want.data(), sizeof(mmb_ksw_job_t) * r.ra->want.size());
-				});
-				// run in chunks to bound the device result buffers; results land in pinned host memory that stays alive until
-				// the end of the batch, so per-read caches just point into it
-				static const int64_t CH = getenv("MM_B200_JOB_CHUNK")? std::max(1, atoi(getenv("MM_B200_JOB_CHUNK"))) : 1 << 20; // test hook: tiny chunks exercise the multi-chunk bookkeeping
-				mmb_ksw_res_t *res = bb.h_res.as<mmb_ksw_res_t>((size_t)n_jobs);
-				// CIGAR arena estimate per job: (qlen+tlen)/2 + 8 operations covers every realistic alignment, the true bound is qlen+tlen
-				// (alternating 1I1D); an overflow is recovered below by rerunning the chunk with the exact size the kernels reported
-				// and growing the host staging buffer. MM_B200_CIG_SHIFT (test hook) shrinks the estimate to force that path.
-				static const int cig_shift = getenv("MM_B200_CIG_SHIFT")? atoi(getenv("MM_B200_CIG_SHIFT")) : 0;
-				// (a spliced job's target spans its introns, each a single N operation: only a query-sized part of the target can turn into operations)
-				auto cig_est = [&](const mmb_ksw_job_t &jb) -> int64_t {
-					if (jb.flag & MMB_JOB_LL) return 0;
-					const int64_t t_eff = (jb.flag & MMB_JOB_SPLICE)? std::min<int64_t>(jb.tlen, 2 * (int64_t)jb.qlen + 64) : jb.tlen;
-					return (((int64_t)jb.qlen + t_eff) / 2 + 8 >> cig_shift) + 1;
-				};
-				int64_t cap_tot = 0;
-				for (int64_t i = 0; i < n_jobs; ++i) cap_tot += cig_est(jobs[i]);
-				while (bb.h_cig.size() <= (size_t)wave) bb.h_cig.emplace_back(new PinBuf);
-				uint32_t *h_cig = bb.h_cig[wave]->as<uint32_t>((size_t)cap_tot + 64);
-				GateHold gatew(G.gated, 1);
-				lap("  gate wait w");
-				std::vector<int64_t> chunk_base; // offset of each chunk's CIGAR block inside h_cig
-				std::vector<const uint32_t*> chunk_dev; // and the block's address in its device arena
-				int64_t cig_fill = 0;
-				for (int64_t b = 0; b < n_jobs; b += CH) {
-					const int64_t m = std::min(CH, n_jobs - b);
-					int64_t cap = 0;
-					for (int64_t i = 0; i < m; ++i) cap += cig_est(jobs[b + i]);
-					for (;;) {
-						mmb_ksw_job_t *d_jobs = bb.jobs.as<mmb_ksw_job_t>((size_t)m);
-						mmb_ksw_res_t *d_res = bb.res.as<mmb_ksw_res_t>((size_t)m);
-						// with the device tail on, every (wave, chunk) keeps its arena until the batch ends (K4 reads the pieces in place);
-						// otherwise one arena is reused, as the host has its copy (spliced jobs reserve room for intron-sized CIGAR estimates)
-						const size_t ki = use_fin? keep_used : 0;
-						while (bb.cig_keep.size() <= ki) bb.cig_keep.emplace_back(new DevBuf);
-						uint32_t *d_cig = bb.cig_keep[ki]->as<uint32_t>((size_t)cap + 4);
-						unsigned long long *d_used = (unsigned long long*)d_cig;
-						MMB_CUDA_CHECK(cudaMemcpyAsync(d_jobs, &jobs[b], sizeof(mmb_ksw_job_t) * m, cudaMemcpyHostToDevice, ctx->stream));
-						MMB_CUDA_CHECK(cudaMemsetAsync(d_used, 0, 8, ctx->stream));
-						mmb_ksw_launch(ctx, &sc, (int)m, &jobs[b], d_jobs, d_seq, B->d_S, 1, d_res, d_cig + 2, cap, d_used);
-						unsigned long long used = 0;
-						MMB_CUDA_CHECK(cudaMemcpyAsync(&res[b], d_res, sizeof(mmb_ksw_res_t) * m, cudaMemcpyDeviceToHost, ctx->stream));
-						MMB_CUDA_CHECK(cudaMemcpyAsync(&used, d_used, 8, cudaMemcpyDeviceToHost, ctx->stream));
-						MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-						if ((int64_t)used > cap) { cap = (int64_t)used + 16; continue; } // rare: rerun the chunk with a larger CIGAR arena
-						if (cig_fill + (int64_t)used > cap_tot) { // grow the wave's host staging buffer, keeping the chunks already staged
-							int64_t rest = 0;
-							for (int64_t i = b + m; i < n_jobs; ++i) rest += cig_est(jobs[i]);
-							const int64_t new_tot = cig_fill + (int64_t)used + rest + 64;
-							std::unique_ptr<PinBuf> nb(new PinBuf);
-							uint32_t *np_ = nb->as<uint32_t>((size_t)new_tot + 64);
-							if (cig_fill) memcpy(np_, h_cig, (size_t)cig_fill * 4);
-							bb.h_cig[wave]->release();
-							bb.h_cig[wave] = std::move(nb);
-							h_cig = np_, cap_tot = new_tot;
-						}
-						ctx->last_d2h_bytes += sizeof(mmb_ksw_res_t) * (uint64_t)m + 4ull * used;
-						ctx->last_h2d_bytes += sizeof(mmb_ksw_job_t) * (uint64_t)m;
-						if (ctx->profiling) ctx->prof_bytes[MMB_PROF_KSW] += 4ull * used;
-						chunk_base.push_back(cig_fill);
-						chunk_dev.push_back(d_cig + 2);
-						++keep_used;
-						if (used) MMB_CUDA_CHECK(cudaMemcpyAsync(h_cig + cig_fill, d_cig + 2, used * 4, cudaMemcpyDeviceToHost, ctx->stream));
-						cig_fill += (int64_t)used;
-						MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-						break;
-					}
-				}
-				gatew.drop();
-				lap("  wave gpu");
-				// hand the results to the per-read caches (pointers only)
-				parallel_for((int64_t)active.size(), n_threads, [&](int64_t t, int) {
-					ReadState &r = rs[active[t]];
-					if (r.done) return;
-					ReadAlign &ra = *r.ra;
-					for (size_t i = 0; i < ra.want.size(); ++i) {
-						const int64_t jid = joff[t] + (int64_t)i;
-						KswDone d; d.r = res[jid], d.cig = h_cig + chunk_base[jid / CH] + res[jid].cigar_off, d.dcig = chunk_dev[jid / CH] + res[jid].cigar_off;
-						ra.done_idx[ra.want_slot[i]] = (int)ra.done.size();
-						ra.done.push_back(d);
-					}
-				});
-			}
-			lap("  wave scatter");
-			for (size_t t = 0; t < active.size(); ++t) if (!rs[active[t]].done) still.push_back(active[t]);
-			if (!still.empty() && n_jobs == 0) { fprintf(stderr, "[ERROR] minimap2_b200: alignment scheduler made no progress\n"); abort(); }
-			active.swap(still);
-			++wave;
+			ctx->last_d2h_bytes += sizeof(mmb_ksw_res_t) * (uint64_t)m + 4ull * used;
+			ctx->last_h2d_bytes += sizeof(mmb_ksw_job_t) * (uint64_t)m;
+			if (ctx->profiling) ctx->prof_bytes[MMB_PROF_KSW] += 4ull * used;
+			chunk_base.push_back(cig_fill);
+			chunk_dev.push_back(d_cig + 2);
+			++b.keep_used;
+			if (used) MMB_CUDA_CHECK(cudaMemcpyAsync(h_cig + cig_fill, d_cig + 2, used * 4, cudaMemcpyDeviceToHost, ctx->stream));
+			cig_fill += (int64_t)used;
+			MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+			break;
 		}
 	}
+	gatew.drop();
+	b.lap("  wave gpu");
+	// hand the results to the per-read caches (pointers only)
+	parallel_for((int64_t)active.size(), b.n_threads, [&](int64_t t, int) {
+		ReadState &r = rs[active[t]];
+		if (r.done) return;
+		ReadAlign &ra = *r.ra;
+		for (size_t i = 0; i < ra.want.size(); ++i) {
+			const int64_t jid = joff[t] + (int64_t)i;
+			KswDone d; d.r = res[jid], d.cig = h_cig + chunk_base[jid / CH] + res[jid].cigar_off, d.dcig = chunk_dev[jid / CH] + res[jid].cigar_off;
+			ra.done_idx[ra.want_slot[i]] = (int)ra.done.size();
+			ra.done.push_back(d);
+		}
+	});
+	return n_jobs;
+}
 
-	lap("waves end");
-	// ---------------- stage 4: finalize (map.c:338-343) ----------------
-	parallel_for(n, n_threads, [&](int64_t j, int) {
+// Stage 3: alignment waves. Every wave replays the driver for each unfinished read, runs the device tail for the reads whose replay
+// is complete, and runs the ksw2 jobs the others asked for.
+static void align_waves(Batch &b)
+{
+	std::vector<ReadState> &rs = b.bb.rs_pool;
+	const mmb_ksw_score_t sc = ksw_score(b.opt);
+	std::vector<int> active;
+	for (int j = 0; j < b.n; ++j) if (!rs[b.live[j]].done) active.push_back(b.live[j]);
+	// The hit-level tail of the driver (CIGAR assembly, mm_fix_cigar, mm_update_extra) runs on the device for finished reads (K4,
+	// finalize.cu) unless the mode needs it on the host (spliced / =X CIGARs / query-strand).
+	const bool use_fin = hl_defer_supported(b.opt);
+	FinPar fpar;
+	for (int i = 0; i < 25; ++i) fpar.mat[i] = sc.mat[i];
+	fpar.q = (int8_t)b.opt->q, fpar.e = (int8_t)b.opt->e, fpar.log_gap = 1;
+	while (!active.empty()) {
+		// replay every active read; collect the jobs they miss
+		parallel_for((int64_t)active.size(), b.n_threads, [&](int64_t t, int) {
+			hl_hp_flush();
+			ReadState &r = rs[active[t]];
+			ReadAlign &ra = *r.ra;
+			ra.want.clear(); ra.want_slot.clear();
+			int n_regs;
+			mm_reg1_t *regs = replay_read(b, r, use_fin, &n_regs);
+			if (ra.defer_abort) { // an inversion probe needs final hit coordinates: this read keeps the whole driver on the host
+				drop_regs(n_regs, regs);
+				regs = replay_read(b, r, false, &n_regs); // jobs the aborted pass asked for stay queued (the full pass asks for a superset)
+			}
+			if (ra.incomplete) drop_regs(n_regs, regs);
+			else if (ra.defer && !ra.fin_hits.empty()) r.n_regs = n_regs, r.regs = regs, r.fin_pending = true;
+			else post_align(b, r, n_regs, regs);
+		});
+		b.lap("  wave replay");
+		device_tail(b, active, fpar);
+		const int64_t n_jobs = ksw_wave(b, active, sc);
+		b.lap("  wave scatter");
+		std::vector<int> still;
+		for (size_t t = 0; t < active.size(); ++t) if (!rs[active[t]].done) still.push_back(active[t]);
+		if (!still.empty() && n_jobs == 0) { fprintf(stderr, "[ERROR] minimap2_b200: alignment scheduler made no progress\n"); abort(); }
+		active.swap(still);
+		++b.wave;
+	}
+}
+
+// Stage 4 (map.c:338-343): MAPQ, and the results to the caller's arrays
+static void finalize_batch(Batch &b, int *n_regs_out, mm_reg1_t **regs_out, int *rep_len_out)
+{
+	std::vector<ReadState> &rs = b.bb.rs_pool;
+	const std::vector<int> &live = b.live;
+	const mm_mapopt_t *opt = b.opt;
+	parallel_for(b.n, b.n_threads, [&](int64_t j, int) {
 		hl_hp_flush();
 		ReadState &r = rs[live[j]];
 		if (r.regs0) free(r.regs0);
@@ -802,59 +920,78 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 		n_regs_out[live[j]] = r.n_regs, regs_out[live[j]] = r.regs;
 		if (rep_len_out) rep_len_out[live[j]] = r.rep_len;
 	});
-	lap("finalize");
-	if (timing) hl_hp_dump("group");
+}
+
+static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *qlens, const char **seqs, const char **names,
+					 int *n_regs_out, mm_reg1_t **regs_out, int *rep_len_out, const mm_mapopt_t *opt, int n_threads, const MapPass &pass)
+{
+	if (n_reads <= 0) return 0;
+	mmb_ctx_t *ctx = G.ctx;
+	Batch b(ctx, G.bb, G.gated, mi, opt, n_threads < 1? 1 : n_threads);
+	mm_idx_bucket_s *B = mi->B;
+	MMB_CUDA_CHECK(cudaSetDevice(ctx->device));
+	// annotated introns of the index (mm_idx_bed_read) for the spliced kernel: what mm_get_junc / mm_idx_bed_junc feed ksw_exts2 (align.c:638-643)
+	ctx->n_junc = B->n_junc, ctx->junc_st = B->d_junc, ctx->junc_en = B->d_junc? B->d_junc + B->n_junc : nullptr;
+	ctx->junc_strand = B->d_junc? (const int8_t*)(B->d_junc + 2 * B->n_junc) : nullptr;
+	for (int t = 0; t < 2; ++t) // splice scores (mm_idx_spsc_read): what mm_idx_spsc_get feeds ksw_exts2 (align.c:640)
+		ctx->n_spsc[t] = B->n_spsc[t], ctx->spsc_pos[t] = (const int64_t*)B->d_spsc[t], ctx->spsc_val[t] = B->d_spsc[t]? B->d_spsc[t] + B->n_spsc[t] * 8 : nullptr;
+	if (!take_reads(b, n_reads, qlens, seqs, names, n_regs_out, regs_out, rep_len_out)) return 0;
+	b.lap("setup");
+	const uint8_t *h_seq = upload_reads(G, b);
+	// the reads are on their way before the group queues for a device slot: every group's upload starts when the batch starts and
+	// overlaps the kernels of the groups ahead of it
+	GateHold gate1(b.gated, 0);
+	b.lap("gate wait 1");
+	seed_batch(b, h_seq, names, pass.occ_cut);
+	b.lap("h2d+sketch+seed+sort");
+	chain_batch(b, pass, gate1);
+	b.lap("chain+rescue+d2h");
+	chains_to_hits(b, pass);
+	if (opt->flag & MM_F_CIGAR) align_waves(b);
+	b.lap("waves end");
+	finalize_batch(b, n_regs_out, regs_out, rep_len_out);
+	b.lap("finalize");
+	if (Lap::on()) hl_hp_dump("group");
 	return 0;
 }
 
-// Kernel-level entry for tests: the seeding stage alone (K1 sketch -> query-side filter -> index lookup -> streak selection ->
-// anchor expansion -> anchor sort, i.e. collect_minimizers + mm_collect_matches + collect_seed_hits of map.c:59-72,168-204) on the
-// context's stream. seqs: the reads back to back (ASCII), off: n_reads+1 offsets. Outputs (host): a_off_out[n_reads+1], rep_len_out,
-// n_mini_out; anchors_xy / mini_pos (if non-null) receive the sorted anchors (16 B each, a_cap entries) and the kept seeds'
-// span<<32|qpos words (mp_cap entries) read after read. Returns the total number of anchors (or -1 if a buffer is too small).
+// Kernel-level entry for tests: the seeding stage alone (seed_batch) on the context's stream. seqs: the reads back to back (ASCII),
+// off: n_reads+1 offsets. Outputs (host): a_off_out[n_reads+1], rep_len_out, n_mini_out; anchors_xy / mini_pos (if non-null) receive
+// the sorted anchors (16 B each, a_cap entries) and the kept seeds' span<<32|qpos words (mp_cap entries) read after read. Returns the
+// total number of anchors (or -1 if a buffer is too small).
 extern "C" int64_t mmb_seed_batch_host(mmb_ctx_t *ctx, const mm_idx_t *mi, int n_reads, const char *seqs, const int64_t *off, int64_t flag, int mid_occ,
 										float q_occ_frac, int max_max_occ, int occ_dist, int64_t *a_off_out, int32_t *rep_len_out, int32_t *n_mini_out,
 										uint64_t *anchors_xy, int64_t a_cap, uint64_t *mini_pos, int64_t mp_cap)
 {
 	if (n_reads <= 0) return 0;
 	MMB_CUDA_CHECK(cudaSetDevice(ctx->device));
-	mm_idx_bucket_s *B = mi->B;
 	static BatchBufs bb; // test entry: one caller at a time
-	const int n = n_reads;
-	const int64_t total_bases = off[n];
-	uint8_t *d_seq = bb.seq.as<uint8_t>((size_t)total_bases + 16);
-	int64_t *d_off = bb.off.as<int64_t>((size_t)n + 1);
-	int32_t *d_qlen = bb.qlen.as<int32_t>((size_t)n);
+	mm_mapopt_t opt; // what seed_batch reads; sdust_thres = 0: no low-complexity masking
+	memset(&opt, 0, sizeof(opt));
+	opt.flag = flag, opt.mid_occ = mid_occ, opt.q_occ_frac = q_occ_frac, opt.max_max_occ = max_max_occ, opt.occ_dist = occ_dist;
+	Batch b(ctx, bb, false, mi, &opt, 1);
+	const int n = b.n = n_reads;
+	b.live.resize(n);
+	for (int j = 0; j < n; ++j) b.live[j] = j;
+	b.off.assign(off, off + n + 1);
+	const int64_t total_bases = b.total_bases = off[n];
+	uint8_t *d_seq = b.d_seq = bb.seq.as<uint8_t>((size_t)total_bases + 16);
+	int64_t *d_off = b.d_off = bb.off.as<int64_t>((size_t)n + 1);
+	int32_t *d_qlen = b.d_qlen = bb.qlen.as<int32_t>((size_t)n);
 	std::vector<int32_t> h_qlen(n);
 	for (int j = 0; j < n; ++j) h_qlen[j] = (int32_t)(off[j + 1] - off[j]);
 	MMB_CUDA_CHECK(cudaMemcpyAsync(d_seq, seqs, total_bases, cudaMemcpyHostToDevice, ctx->stream));
 	MMB_CUDA_CHECK(cudaMemcpyAsync(d_off, off, sizeof(int64_t) * (n + 1), cudaMemcpyHostToDevice, ctx->stream));
 	MMB_CUDA_CHECK(cudaMemcpyAsync(d_qlen, h_qlen.data(), sizeof(int32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
 	if (total_bases > 0) encode_kernel<<<(unsigned)((total_bases / 4 + 256) / 256), 256, 0, ctx->stream>>>(d_seq, total_bases);
-	int64_t *d_mz_off = bb.mz_off.as<int64_t>((size_t)n + 1);
-	const int64_t total_mz = mmb_sketch_device(ctx, d_seq, nullptr, d_off, n, nullptr, 0, mi->w, mi->k, mi->flag & MM_I_HPC, total_bases, bb.mz, d_mz_off, bb.t1, bb.t2, 1);
-	SeedArgs S;
-	S.ix = B->view(mi), S.n_reads = n, S.mz = (m128*)bb.mz.p, S.mz_off = d_mz_off, S.qlen = d_qlen;
-	S.n_mz = bb.n_mz.as<int32_t>((size_t)n);
-	S.q_occ_max = mid_occ, S.q_occ_frac = q_occ_frac, S.max_occ = mid_occ, S.max_max_occ = max_max_occ, S.occ_dist = occ_dist, S.flag = flag;
-	const size_t nm = (size_t)total_mz + 4;
-	S.s_n = bb.s_n.as<uint32_t>(nm), S.s_off = bb.s_off.as<uint64_t>(nm), S.k_idx = bb.k_idx.as<uint32_t>(nm), S.k_aoff = bb.k_aoff.as<uint32_t>(nm);
-	S.flt = bb.flt.as<uint8_t>(nm), S.mini_pos = bb.mini_pos.as<uint64_t>(nm);
-	S.n_keep = bb.n_keep.as<int32_t>((size_t)n), S.rep_len = bb.rep_len.as<int32_t>((size_t)n), S.n_a = bb.n_a.as<int64_t>((size_t)n + 1);
-	init_nmz_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_mz_off, n, S.n_mz);
-	if (flag & (MM_F_FOR_ONLY | MM_F_REV_ONLY)) S.k_cnt = bb.k_cnt.as<uint32_t>(nm); // skip_seed's strand rule (no query names here: no name tests)
-	mmb_seed_select_device(ctx, S, total_mz);
-	int64_t *d_a_off = bb.a_off.as<int64_t>((size_t)n + 1);
-	copy_i64_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(S.n_a, n, d_a_off);
-	const int64_t total_a = mmb_exclusive_scan_i64(ctx, d_a_off, n, true);
-	S.a = bb.a.as<m128>((size_t)total_a + 4), S.a_off = d_a_off;
-	S.a_sorted = bb.a2.as<m128>((size_t)total_a + 4);
-	mmb_seed_expand_sort_device(ctx, S, total_mz, total_a, bb.stk);
+	seed_batch(b, (const uint8_t*)seqs, nullptr, mid_occ);
+	const SeedArgs &S = b.S;
+	const int64_t total_a = b.total_a;
 	std::vector<int64_t> h_mz_off((size_t)n + 1);
-	MMB_CUDA_CHECK(cudaMemcpyAsync(a_off_out, d_a_off, sizeof(int64_t) * (n + 1), cudaMemcpyDeviceToHost, ctx->stream));
+	MMB_CUDA_CHECK(cudaMemcpyAsync(a_off_out, S.a_off, sizeof(int64_t) * (n + 1), cudaMemcpyDeviceToHost, ctx->stream));
 	MMB_CUDA_CHECK(cudaMemcpyAsync(rep_len_out, S.rep_len, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
 	MMB_CUDA_CHECK(cudaMemcpyAsync(n_mini_out, S.n_keep, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, ctx->stream));
-	MMB_CUDA_CHECK(cudaMemcpyAsync(h_mz_off.data(), d_mz_off, sizeof(int64_t) * (n + 1), cudaMemcpyDeviceToHost, ctx->stream));
+	MMB_CUDA_CHECK(cudaMemcpyAsync(h_mz_off.data(), S.mz_off, sizeof(int64_t) * (n + 1), cudaMemcpyDeviceToHost, ctx->stream));
 	MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
 	if (anchors_xy) {
 		if (total_a > a_cap) return -1;
@@ -877,7 +1014,7 @@ void mmb_register_ctx(mmb_ctx_t *c);
 
 static int g_groups_override = 0;
 extern "C" void mmb_set_gpu_slots(int n) { g_gpu_slots = n < 1? 1 : n; }
-extern "C" void mmb_set_groups(int n) { g_groups_override = n; } // 0 = default (MM_B200_GROUPS or 3)
+extern "C" void mmb_set_groups(int n) { g_groups_override = n; } // 0 = default (MM_B200_GROUPS or 12); negative: that many groups, one after another
 
 static GroupCtx &get_group(int g, int device)
 {
@@ -899,7 +1036,6 @@ static GroupCtx &get_group(int g, int device)
 static int map_batch_pass(const mm_idx_t *mi, int n_reads, const int *qlens, const char **seqs, const char **names,
 						  int *n_regs_out, mm_reg1_t **regs_out, int *rep_len_out, const mm_mapopt_t *opt, int n_threads, const MapPass &pass)
 {
-	auto sub = [&](int b) { MapPass p = pass; if (p.no_chain) p.no_chain += b; return p; }; // the pass as a group starting at read b sees it
 	static int ng_env = getenv("MM_B200_GROUPS")? atoi(getenv("MM_B200_GROUPS")) : 12;
 	const bool sequential = g_groups_override < 0; // negative override: same groups, run one after another (clean per-kernel timing)
 	const int ng_req = g_groups_override > 0? g_groups_override : g_groups_override < 0? -g_groups_override : ng_env;
@@ -915,13 +1051,7 @@ static int map_batch_pass(const mm_idx_t *mi, int n_reads, const int *qlens, con
 		// equal shares, except that the last three groups shrink (3/4, 1/2, 1/4 of a share): the end of the batch is then
 		// the short serial chain of a small group instead of a full-size one
 		std::vector<double> wsum(NG + 1, 0.0);
-		// MM_B200_TAPER (development): comma-separated shares of the last groups, e.g. "0.7,0.45,0.25,0.12"
-		static const std::vector<double> taper = []() { std::vector<double> t; const char *e = getenv("MM_B200_TAPER"); if (e) { for (const char *p = e; *p;) { char *q; t.push_back(strtod(p, &q)); p = *q == ','? q + 1 : q; if (q == p && *q != ',') break; } } return t; }();
-		for (int g2 = 0; g2 < NG; ++g2) {
-			double wgt = NG >= 8 && g2 >= NG - 3? 0.25 * (NG - g2) : 1.0;
-			if (!taper.empty() && NG >= 8) wgt = g2 >= NG - (int)taper.size()? taper[g2 - (NG - (int)taper.size())] : 1.0;
-			wsum[g2 + 1] = wsum[g2] + wgt;
-		}
+		for (int g2 = 0; g2 < NG; ++g2) wsum[g2 + 1] = wsum[g2] + (NG >= 8 && g2 >= NG - 3? 0.25 * (NG - g2) : 1.0);
 		int64_t acc = 0; int g = 1;
 		for (int i = 0; i < n_reads && g < NG; ++i) {
 			acc += qlens[i] > 0? qlens[i] : 0;
@@ -930,21 +1060,19 @@ static int map_batch_pass(const mm_idx_t *mi, int n_reads, const int *qlens, con
 		for (; g < NG; ++g) cut[g] = n_reads;
 		cut[NG] = n_reads;
 	}
+	auto run_group = [&](int g) {
+		const int b = cut[g], m = cut[g + 1] - cut[g];
+		MapPass p = pass; // the pass as a group starting at read b sees it
+		if (p.no_chain) p.no_chain += b;
+		if (m > 0) map_group(get_group(g, device), mi, m, qlens + b, seqs + b, names? names + b : nullptr, n_regs_out + b, regs_out + b,
+							 rep_len_out? rep_len_out + b : nullptr, opt, n_threads, p);
+	};
 	if (sequential) {
-		for (int g = 0; g < NG; ++g) {
-			const int b = cut[g], m = cut[g + 1] - cut[g];
-			if (m > 0) map_group(get_group(g, device), mi, m, qlens + b, seqs + b, names? names + b : nullptr, n_regs_out + b, regs_out + b,
-								 rep_len_out? rep_len_out + b : nullptr, opt, n_threads, sub(b));
-		}
+		for (int g = 0; g < NG; ++g) run_group(g);
 		return 0;
 	}
 	std::vector<std::thread> th;
-	for (int g = 0; g < NG; ++g)
-		th.emplace_back([&, g]() {
-			const int b = cut[g], m = cut[g + 1] - cut[g];
-			if (m > 0) map_group(get_group(g, device), mi, m, qlens + b, seqs + b, names? names + b : nullptr, n_regs_out + b, regs_out + b,
-								 rep_len_out? rep_len_out + b : nullptr, opt, n_threads, sub(b));
-		});
+	for (int g = 0; g < NG; ++g) th.emplace_back(run_group, g);
 	for (auto &x : th) x.join();
 	return 0;
 }

@@ -916,37 +916,29 @@ void mmb_seed_expand_sort_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz, 
 		++ctx->n_launch;
 		int *d_tie_cnt = d_cls_cnt + N_CLS + 1, *d_tie_list = d_cls_list + (size_t)(N_CLS + 1) * A.n_reads;
 		int *d_fb_cnt = d_cls_cnt + N_CLS + 2, *d_fb_list = d_cls_list + (size_t)(N_CLS + 2) * A.n_reads;
-		static const bool use_bitonic = getenv("MM_B200_SORT_BITONIC") != nullptr; // development switch: the network sort for every read
-		if (!use_bitonic) {
-			#define MMB_RADIX_LAUNCH(CAP_, NT_, c_) do { \
-				const size_t smem_ = (size_t)(CAP_) * 12 + (size_t)256 * ((NT_) / 32 + 1) * 2; \
-				{ static std::once_flag once_; std::call_once(once_, [&]() { MMB_CUDA_CHECK(cudaFuncSetAttribute(sort_radix_kernel<CAP_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_)); }); } \
-				int per_sm_ = 1; \
-				MMB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_, sort_radix_kernel<CAP_, NT_>, NT_, smem_)); \
-				sort_radix_kernel<CAP_, NT_><<<ctx->n_sm * (per_sm_ > 0? per_sm_ : 1), NT_, smem_, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_cls_list + (size_t)(c_) * A.n_reads, \
-					d_cls_cnt + (c_), d_tie_cnt, d_tie_list, d_fb_cnt, d_fb_list); \
-				++ctx->n_launch; } while (0)
-			MMB_RADIX_LAUNCH(1024, 128, 0);
-			MMB_RADIX_LAUNCH(2048, 256, 1);
-			MMB_RADIX_LAUNCH(4096, 512, 2);
-			MMB_RADIX_LAUNCH(8192, 512, 3); // 16 elements per thread, 64 registers: two CTAs per SM instead of one 1024-thread CTA that owns the whole register file
-			MMB_RADIX_LAUNCH(16384, 1024, 4);
-			#undef MMB_RADIX_LAUNCH
-		}
-		{ // network sort: the fallback of the radix kernels (keys differing in more than 33 bit positions), or everything under the switch
-			int cap = CAP0;
-			for (int c = 0; c < N_CLS; ++c, cap <<= 1) {
-				if (!use_bitonic && c < N_CLS - 1) continue; // fallback list: one launch with the largest class
-				const size_t smem = (size_t)cap * 10;
-				const int threads = cap >= 8192? 1024 : cap >= 2048? 512 : 256;
-				{ static std::once_flag once; std::call_once(once, [&]() { MMB_CUDA_CHECK(cudaFuncSetAttribute(sort_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->smem_optin - 1024)); }); }
-				int per_sm = 1;
-				MMB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sort_block_kernel, threads, smem));
-				const int grid = ctx->n_sm * (per_sm > 0? per_sm : 1);
-				sort_block_kernel<<<grid, threads, smem, ctx->stream>>>(A.a, A.a_sorted, A.a_off, use_bitonic? d_cls_list + (size_t)c * A.n_reads : d_fb_list,
-																		 use_bitonic? d_cls_cnt + c : d_fb_cnt, cap, d_tie_cnt, d_tie_list);
-				++ctx->n_launch;
-			}
+		#define MMB_RADIX_LAUNCH(CAP_, NT_, c_) do { \
+			const size_t smem_ = (size_t)(CAP_) * 12 + (size_t)256 * ((NT_) / 32 + 1) * 2; \
+			{ static std::once_flag once_; std::call_once(once_, [&]() { MMB_CUDA_CHECK(cudaFuncSetAttribute(sort_radix_kernel<CAP_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_)); }); } \
+			int per_sm_ = 1; \
+			MMB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_, sort_radix_kernel<CAP_, NT_>, NT_, smem_)); \
+			sort_radix_kernel<CAP_, NT_><<<ctx->n_sm * (per_sm_ > 0? per_sm_ : 1), NT_, smem_, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_cls_list + (size_t)(c_) * A.n_reads, \
+				d_cls_cnt + (c_), d_tie_cnt, d_tie_list, d_fb_cnt, d_fb_list); \
+			++ctx->n_launch; } while (0)
+		MMB_RADIX_LAUNCH(1024, 128, 0);
+		MMB_RADIX_LAUNCH(2048, 256, 1);
+		MMB_RADIX_LAUNCH(4096, 512, 2);
+		MMB_RADIX_LAUNCH(8192, 512, 3); // 16 elements per thread, 64 registers: two CTAs per SM instead of one 1024-thread CTA that owns the whole register file
+		MMB_RADIX_LAUNCH(16384, 1024, 4);
+		#undef MMB_RADIX_LAUNCH
+		{ // network sort: the fallback of the radix kernels (keys differing in more than 33 bit positions), one launch sized for the largest class
+			const int cap = CAP0 << (N_CLS - 1), threads = 1024;
+			const size_t smem = (size_t)cap * 10;
+			{ static std::once_flag once; std::call_once(once, [&]() { MMB_CUDA_CHECK(cudaFuncSetAttribute(sort_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->smem_optin - 1024)); }); }
+			int per_sm = 1;
+			MMB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sort_block_kernel, threads, smem));
+			const int grid = ctx->n_sm * (per_sm > 0? per_sm : 1);
+			sort_block_kernel<<<grid, threads, smem, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_fb_list, d_fb_cnt, cap, d_tie_cnt, d_tie_list);
+			++ctx->n_launch;
 		}
 		// exact emulation: reads with equal keys go through the shared-memory walker (cap 15360 anchors: 12 B/entry + per-lane bucket tables);
 		// whatever does not fit, and the oversize class, falls back to the global-memory walker (one thread per read)

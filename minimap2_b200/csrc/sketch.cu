@@ -512,8 +512,7 @@ int64_t mmb_sketch_device(mmb_ctx_t *ctx, const uint8_t *d_bytes, const uint32_t
 	if (n_seq <= 0) return 0;
 	if (!(w > 0 && w < 256 && k > 0 && k <= 28)) { fprintf(stderr, "[ERROR] mm_sketch: invalid w=%d k=%d\n", w, k); abort(); }
 	ProfScope prof(ctx, MMB_PROF_SKETCH, (uint64_t)total_bases);
-	static const bool force_chunk = getenv("MM_B200_SKETCH_CHUNK") != nullptr; // development switch: the chunk-replay kernel for everything
-	if ((k & 1) && w + k <= SKT_HALO && !is_hpc && total_bases > 0 && !force_chunk) { // tile kernel over 2-bit-packed bases (see above)
+	if ((k & 1) && w + k <= SKT_HALO && !is_hpc && total_bases > 0) { // tile kernel over 2-bit-packed bases (see above)
 		DevBuf &pkb = ctx->sk_pk, &nmb = ctx->sk_nm, &misc = ctx->sk_misc; // per context (= per scheduler group); sized once in steady state
 		const int64_t nw32 = (total_bases + 31) / 32;
 		uint32_t *d_pk = pkb.as<uint32_t>((size_t)nw32 * 2 + 64), *d_nm = nmb.as<uint32_t>((size_t)nw32 + 64);
