@@ -47,6 +47,7 @@ struct KswArgs {
 	int L, LQ;             // state array length (multiple of 16) / reversed-query length (multiple of 16)
 	int8_t mat[25];
 	int8_t q, e, q2, e2;   // already ordered so that q+e <= q2+e2
+	int qe0;               // q+e as the caller gave them, before that reordering: H(0,0) = v - qe0 (ksw2_extd2_sse.c:68,358,379)
 	int8_t skip;           // -min(mat) > 2(q+e): the reference returns immediately (:100)
 	int long_thres, long_diff;
 	int8_t sp[4];          // spliced variant: penalties of the four signal classes (ksw2_exts2_sse.c:113-121)
@@ -510,7 +511,7 @@ __global__ void __launch_bounds__(256, KE_MINB) ksw_extd2_kernel(KswArgs A)
 					else if (brank <= 4 * nblk) { int k = brank - 1; max_t = st0 + (k % nblk) * 4 + k / nblk; }
 					else max_t = en1 + (brank - 1 - 4 * nblk);
 				} else {
-					if (g == 0) H[0] = (int8_t)vn[0] - qe;
+					if (g == 0) H[0] = (int8_t)vn[0] - A.qe0;
 					gsync<G>();
 					max_H = H[0], max_t = 0;
 				}
@@ -534,7 +535,7 @@ __global__ void __launch_bounds__(256, KE_MINB) ksw_extd2_kernel(KswArgs A)
 							if (d0 > d1) H0 += d0; else H0 += d1, ++last_H0_t;
 						} else if (last_H0_t >= st0 && last_H0_t <= en0) H0 += (int8_t)vn[last_H0_t];
 						else ++last_H0_t, H0 += (int8_t)u[last_H0_t];
-					} else H0 = (int8_t)vn[0] - qe, last_H0_t = 0;
+					} else H0 = (int8_t)vn[0] - A.qe0, last_H0_t = 0;
 				}
 				if (flag & MMB_KSW_APPROX_DROP) { // not used by align.c; supported for API completeness
 					int hh = __shfl_sync(0xffffffffu, H0, 0), tt = __shfl_sync(0xffffffffu, last_H0_t, 0);
@@ -716,6 +717,7 @@ void mmb_ksw_launch(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, int n_jobs, const
 	A.cigar = d_cigar, A.cigar_cap = cigar_cap, A.cigar_used = d_cigar_used;
 	for (int i = 0; i < 25; ++i) A.mat[i] = sc->mat[i];
 	int8_t q = sc->q, e = sc->e, q2 = sc->q2, e2 = sc->e2;
+	A.qe0 = q + e; // the same in both passes: ksw_exts2_sse does not reorder (ksw2_exts2_sse.c:65)
 	if (q2 + e2 < q + e) std::swap(q, q2), std::swap(e, e2); // ksw2_extd2_sse.c:78
 	A.q = q, A.e = e, A.q2 = q2, A.e2 = e2;
 	int min_sc = sc->mat[1];

@@ -42,7 +42,9 @@ struct FastArgs {
 	int qmax;                             // shared-memory query staging capacity per warp
 	int8_t mch, mis, scn;
 	int8_t q, e, q2, e2;
+	int qe0;                              // q+e before the (q,e)/(q2,e2) reordering: H(0,0) = v - qe0 (ksw2_extd2_sse.c:68,358)
 	int8_t zd_q, zd_e;                    // gap open/extension as mm_test_zdrop uses them (opt->q, opt->e: not reordered)
+	int8_t zd_scn;                        // that scan's score for an ambiguous base: the matrix entry, also when it is 0 and the DP scores -e2
 	int zd_skip;                          // > 0: skip that scan when the path's total penalty cannot exceed it (mmb_ksw_score_t::zd_skip)
 	int long_thres, long_diff;
 	int8_t mat[25];
@@ -187,7 +189,7 @@ __global__ void __launch_bounds__(128) ksw_fast_kernel(FastArgs A)
 					#pragma unroll
 					for (int c = 0; c < C; ++c) if (t0 + c >= 1 && t0 + c < tlen) hrow += u[c];
 				}
-				if (lane == 0) hcol0 += j == 0? hc0 - qe : hc0; // H(0,0) = v - (q+e) (:366); then H(0,j) = H(0,j-1) + v(0,j)
+				if (lane == 0) hcol0 += j == 0? hc0 - A.qe0 : hc0; // H(0,0) = v - (q+e) (:358, q+e as given); then H(0,j) = H(0,j-1) + v(0,j)
 				pk_prev = (vl & 0xff) | (xl & 0xff) << 8 | (x2l & 0xff) << 16;
 				uint8_t *prow = p + (size_t)j * W + lane * CP;
 				if (CP == 4) *(uint32_t*)prow = dw[0];
@@ -477,7 +479,7 @@ __global__ void __launch_bounds__(128, PK_MINB) ksw_pk_kernel(FastArgs A)
 		int score = hrow;
 		#pragma unroll
 		for (int o = LN / 2; o > 0; o >>= 1) score += __shfl_xor_sync(full, score, o);
-		score += (int)(hcol_acc >> 8) - 128 * qlen - qe;
+		score += (int)(hcol_acc >> 8) - 128 * qlen - A.qe0;
 		score = __shfl_sync(full, score, lead);
 		__syncwarp();
 		// ---- traceback from (tlen-1, qlen-1) (ksw2.h:130-162; no forced states: the band is never clipped) ----
@@ -563,7 +565,7 @@ __global__ void __launch_bounds__(128, PK_MINB) ksw_pk_kernel(FastArgs A)
 			else if (g_flag & MMB_JOB_ZDROP) {
 				const uint8_t *gq = smem + (size_t)(wk * NJ + g) * A.qmax;
 				const uint8_t *gt = smem + (size_t)nwk * NJ * A.qmax + (size_t)(wk * NJ + g) * TSM;
-				const int zq = A.zd_q, ze = A.zd_e, mch = A.mch, mis = A.mis, scn = A.scn;
+				const int zq = A.zd_q, ze = A.zd_e, mch = A.mch, mis = A.mis, scn = A.zd_scn;
 				int sco = 0, mx = INT32_MIN, mi = -1, mj = -1, ti0 = 0, qj0 = 0;
 				zd_max = 0;
 				for (int k = n - 1; k >= 0; --k) {
@@ -683,9 +685,10 @@ void mmb_ksw_fast_plan(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, const std::vec
 	A.jobs = d_jobs, A.query = d_query, A.target = d_target, A.t_packed = t_packed, A.res = d_res;
 	A.cigar = d_cigar, A.cigar_cap = cigar_cap, A.cigar_used = d_cigar_used;
 	int8_t q = sc->q, e = sc->e, q2 = sc->q2, e2 = sc->e2;
+	A.qe0 = q + e;
 	if (q2 + e2 < q + e) std::swap(q, q2), std::swap(e, e2);
 	A.q = q, A.e = e, A.q2 = q2, A.e2 = e2;
-	A.zd_q = sc->q, A.zd_e = sc->e, A.zd_skip = sc->zd_skip;
+	A.zd_q = sc->q, A.zd_e = sc->e, A.zd_scn = sc->mat[24], A.zd_skip = sc->zd_skip;
 	A.one = 1u, A.neg1 = 0xffffffffu;
 	A.mch = sc->mat[0], A.mis = sc->mat[1], A.scn = sc->mat[24] == 0? (int8_t)(-e2) : sc->mat[24];
 	for (int i = 0; i < 25; ++i) A.mat[i] = sc->mat[i];

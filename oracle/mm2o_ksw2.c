@@ -80,6 +80,7 @@ void mm2o_extd2(int qlen, const uint8_t *query, int tlen, const uint8_t *target,
 				int q_, int e_, int q2_, int e2_, int w, int zdrop, int end_bonus, int flag, mm2o_ez_t *ez)
 {
 	int8_t q = I8(q_), e = I8(e_), q2 = I8(q2_), e2 = I8(e2_);
+	const int qe0 = q + e; /* :68: taken before the swap below, so H(0,0) keeps the caller's first gap pair */
 	int r, t, n_col, tlen16, qlen16, last_st, last_en, max_sc, min_sc, long_thres, long_diff;
 	int with_cigar = !(flag & MM2O_EZ_SCORE_ONLY), approx_max = !!(flag & MM2O_EZ_APPROX_MAX), right = !!(flag & MM2O_EZ_RIGHT);
 	int8_t *u, *v, *x, *y, *x2, *y2, *s, *ou, *ov, *ox, *oy, *ox2, *oy2;
@@ -225,7 +226,7 @@ void mm2o_extd2(int qlen, const uint8_t *query, int tlen, const uint8_t *target,
 					H[t] += (int32_t)v[t];
 					if (H[t] > max_H) max_H = H[t], max_t = t;
 				}
-			} else H[0] = v[0] - qe, max_H = H[0], max_t = 0;
+			} else H[0] = v[0] - qe0, max_H = H[0], max_t = 0; /* :358 */
 			if (en0 == tlen - 1 && H[en0] > ez->mte) ez->mte = H[en0], ez->mte_q = r - en0;
 			if (r - st0 == qlen - 1 && H[st0] > ez->mqe) ez->mqe = H[st0], ez->mqe_t = st0;
 			if (apply_zdrop_rot(ez, max_H, r, max_t, zdrop, e2)) break;
@@ -241,7 +242,7 @@ void mm2o_extd2(int qlen, const uint8_t *query, int tlen, const uint8_t *target,
 				} else {
 					++last_H0_t, H0 += u[last_H0_t];
 				}
-			} else H0 = v[0] - qe, last_H0_t = 0;
+			} else H0 = v[0] - qe0, last_H0_t = 0; /* :379 */
 			if ((flag & MM2O_EZ_APPROX_DROP) && apply_zdrop_rot(ez, H0, r, last_H0_t, zdrop, e2)) break;
 			if (r == qlen + tlen - 2 && en0 == tlen - 1) ez->score = H0;
 		}

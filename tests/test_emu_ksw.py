@@ -124,11 +124,11 @@ def test_emulated_kernels_match_oracle(emu):
     assert n_zd >= 20
 
 
-def small_spliced_pair(rng, n_exon, err, introns_out=None):
+def small_spliced_pair(rng, n_exon, err, introns_out=None, intron_len=(30, 200)):
     ex = [rng.integers(0, 4, int(rng.integers(20, 90))).astype(np.uint8) for _ in range(n_exon)]
     parts = [ex[0]]; pos = len(ex[0])
     for k in range(1, n_exon):
-        intron = rng.integers(0, 4, int(rng.integers(30, 200))).astype(np.uint8)
+        intron = rng.integers(0, 4, int(rng.integers(*intron_len))).astype(np.uint8)
         sig = int(rng.integers(0, 5))
         if sig < 3: intron[:2] = [2, 3]; intron[-2:] = [0, 2]
         elif sig == 3: intron[:2] = [2, 1]; intron[-2:] = [0, 2]

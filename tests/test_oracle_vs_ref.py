@@ -58,6 +58,42 @@ def test_extd2_other_scoring_and_generic():
             assert x == y, (a_, b_, it, w, flag)
 
 
+@pytest.mark.parametrize("scoring", [(2, 4, 4, 2, 24, 1, 0), (2, 4, 4, 2, 24, 1, 2), (2, 4, 24, 1, 4, 2, 1), (2, 5, 4, 2, 56, 1, 1)],
+                         ids=["sc_ambi0", "sc_ambi2", "swapped-gaps", "packed-limit"])
+def test_extd2_scoring_regimes(scoring):
+    """the regimes with their own code in the kernels: a 0 ambiguous-base score (scored -e2 by ksw_extd2_sse), sc_ambi 2, gap costs given
+    in the order the reference swaps (q2+e2 < q+e), and the packed kernel's last scoring; N-rich sequences"""
+    a_, b_, q, e, q2, e2, ambi = scoring
+    mat = O.simple_mat(a_, b_, ambi)
+    rng = np.random.default_rng(sum(scoring))
+    for it in range(120):
+        qq, tt = rand_pair(rng, int(rng.integers(1, 350)), err=float(rng.choice([0.02, 0.1, 0.25])))
+        for s in (qq, tt):
+            s[rng.random(len(s)) < float(rng.choice([0.02, 0.1]))] = 4
+        w = int(rng.choice([-1, 17, 100, 751, 30001]))
+        flag = int(rng.choice([0, APPROX, EXT, EXT | RIGHT | REVC, RIGHT, 0x01]))
+        zd = int(rng.choice([-1, 100, 400]))
+        x = O.oracle_extd2(qq, tt, mat, q, e, q2, e2, w, zd, -1, flag)
+        y = O.ref_extd2(qq, tt, mat, q, e, q2, e2, w, zd, -1, flag)
+        assert x == y, (scoring, it, w, flag)
+
+
+@pytest.mark.parametrize("scoring", [(1, 2, 2, 1, 32, 0), (1, 4, 2, 1, 32, 2), (2, 5, 4, 2, 56, 1)], ids=["sc_ambi0", "sc_ambi2", "packed-limit"])
+def test_exts2_scoring_regimes(scoring):
+    """ksw_exts2_sse with sc_ambi 0 (ambiguous bases scored -e), sc_ambi 2 and the packed kernel's last scoring, N-rich spliced pairs"""
+    a_, b_, q, e, q2, ambi = scoring
+    rng = np.random.default_rng(40 + sum(scoring))
+    mat = O.simple_mat(a_, b_, ambi)
+    for it in range(80):
+        qq, tt = _spliced_pair(rng, int(rng.integers(1, 4)), 0.05)
+        for s in (qq, tt):
+            s[rng.random(len(s)) < 0.08] = 4
+        fl = int(rng.choice([0, 0x08, 0x40, 0x40 | 0x02 | 0x80, 0x02])) | int(rng.choice([0x100, 0x200])) | int(rng.choice([0, 0x400, 0x400 | 0x800]))
+        x = O.oracle_exts2(qq, tt, mat, q, e, q2, 9, 200, -1, 9, 5, fl)
+        y = O.ref_exts2(qq, tt, mat, q, e, q2, 9, 200, -1, 9, 5, fl)
+        assert x == y, (scoring, it, hex(fl))
+
+
 def test_extd2_long_band_limited():
     """end-extension shape: long sequences, w=751 so the band limits st0/en0 and 16-lane edge artefacts are live"""
     rng = np.random.default_rng(11)
