@@ -15,6 +15,21 @@
 
 #define KSW_NEG_INF_H (-0x40000000)
 
+void hl_gen_mat(int8_t *mat, const mm_mapopt_t *opt) // align.c:11-38 (m = 5)
+{
+	const int m = 5;
+	int8_t aa = (int8_t)(opt->a < 0? -opt->a : opt->a), bb = (int8_t)(opt->b > 0? -opt->b : opt->b);
+	int8_t sa = (int8_t)(opt->sc_ambi > 0? -opt->sc_ambi : opt->sc_ambi);
+	for (int i = 0; i < m - 1; ++i) {
+		for (int j = 0; j < m - 1; ++j) mat[i * m + j] = i == j? aa : bb;
+		mat[i * m + m - 1] = sa;
+	}
+	for (int j = 0; j < m; ++j) mat[(m - 1) * m + j] = sa;
+	if (opt->transition == 0 || opt->transition == opt->b) return;
+	int8_t t = (int8_t)(opt->transition > 0? -opt->transition : opt->transition);
+	mat[0 * m + 2] = t, mat[1 * m + 3] = t, mat[2 * m + 0] = t, mat[3 * m + 1] = t;
+}
+
 namespace {
 
 struct Ez {
@@ -40,20 +55,6 @@ struct Seg { // a piece of the query (on strand `rev`, strand coordinates) and o
 
 inline uint32_t roundup32(uint32_t x) { --x; x |= x >> 1; x |= x >> 2; x |= x >> 4; x |= x >> 8; x |= x >> 16; return ++x; }
 
-void gen_mat(int8_t *mat, int a, int b, int transition, int sc_ambi) // align.c:11-38 (m = 5)
-{
-	const int m = 5;
-	int8_t aa = (int8_t)(a < 0? -a : a), bb = (int8_t)(b > 0? -b : b), sa = (int8_t)(sc_ambi > 0? -sc_ambi : sc_ambi);
-	for (int i = 0; i < m - 1; ++i) {
-		for (int j = 0; j < m - 1; ++j) mat[i * m + j] = i == j? aa : bb;
-		mat[i * m + m - 1] = sa;
-	}
-	for (int j = 0; j < m; ++j) mat[(m - 1) * m + j] = sa;
-	if (transition == 0 || transition == b) return;
-	int8_t t = (int8_t)(transition > 0? -transition : transition);
-	mat[0 * m + 2] = t, mat[1 * m + 3] = t, mat[2 * m + 0] = t, mat[3 * m + 1] = t;
-}
-
 struct Driver {
 	const mm_mapopt_t *opt;
 	const mm_idx_t *mi;
@@ -63,7 +64,7 @@ struct Driver {
 	bool pending; // set while walking a region whose results are not all available
 
 	Driver(const mm_mapopt_t *o, const mm_idx_t *m, ReadAlign &r) : opt(o), mi(m), ra(r), qlen(r.qlen), pending(false) {
-		gen_mat(mat, o->a, o->b, o->transition, o->sc_ambi);
+		hl_gen_mat(mat, o);
 	}
 
 	KswKey make_key(const Seg &s, int w, int zdrop, int end_bonus, int flag) const {
@@ -365,111 +366,70 @@ struct Driver {
 	void update_extra(mm_reg1_t *r, const uint8_t *qseq, const uint8_t *tseq, int8_t q, int8_t e, int is_eqx, int log_gap) { // align.c:254-303
 		HpScope hp_(HP_EXTRA);
 		int32_t qshift, tshift, toff = 0, qoff = 0;
-		double s = 0.0, max = 0.0;
 		mm_extra_t *p = r->p;
 		if (p == 0) return;
 		fix_cigar(r, qseq, tseq, &qshift, &tshift);
 		qseq += qshift, tseq += tshift;
-		// The running score s of align.c:266-297 is a sum of integers (matrix entries, q) and of e * mg_log2(1+len) terms whose
-		// float mantissa keeps them multiples of 2^-32 in any realistic range, so the reference's double arithmetic is exact
-		// and a 2^-32 fixed-point integer reproduces it; the double loop below remains as the fallback when a gap penalty is
-		// not representable.
-		bool fixed_ok = true;
-		{
-			int64_t matfx[25];
-			for (int i = 0; i < 25; ++i) matfx[i] = (int64_t)mat[i] << 32;
-			int64_t sfx = 0, maxfx = 0;
-			const int64_t afx = matfx[0];
-			const bool diag_ok = mat[0] > 0 && mat[6] == mat[0] && mat[12] == mat[0] && mat[18] == mat[0]; // one positive match score
-			int32_t blen = 0, mlen = 0, n_ambi_tot = 0, is_spliced = 0;
-			toff = qoff = 0;
-			for (uint32_t k = 0; k < p->n_cigar && fixed_ok; ++k) {
-				uint32_t op = p->cigar[k] & 0xf, len = p->cigar[k] >> 4;
-				if (op == MM_CIGAR_MATCH) {
-					int n_ambi = 0, n_diff = 0;
-					const uint8_t *pq = qseq + qoff, *pt = tseq + toff;
-					if (diag_ok) {
-						// runs of identical unambiguous bases add run * a at once (the running score only rises there, so
-						// testing the maximum at the end of the run is the same as testing it at every base); 16 bases
-						// per comparison, both buffers carry 16 bytes of slack
-						for (uint32_t l0 = 0; l0 < len; l0 += 16) {
-							const uint32_t nb = len - l0 < 16? len - l0 : 16;
-							const __m128i vq = _mm_loadu_si128((const __m128i*)(pq + l0)), vt = _mm_loadu_si128((const __m128i*)(pt + l0));
-							const __m128i same = _mm_cmpeq_epi8(vq, vt), amb = _mm_cmpgt_epi8(_mm_or_si128(vq, vt), _mm_set1_epi8(3));
-							uint32_t ev = (uint32_t)_mm_movemask_epi8(_mm_or_si128(amb, _mm_xor_si128(same, _mm_set1_epi8(-1)))) & ((1u << nb) - 1);
-							uint32_t pos = 0;
-							while (ev) {
-								const uint32_t b = (uint32_t)__builtin_ctz(ev);
-								if (b > pos) { sfx += (int64_t)(b - pos) * afx; maxfx = maxfx > sfx? maxfx : sfx; }
-								const int cq = pq[l0 + b], ct = pt[l0 + b];
-								if ((ct | cq) > 3) ++n_ambi; else ++n_diff;
-								sfx += matfx[ct * 5 + cq];
-								if (sfx < 0) sfx = 0;
-								else maxfx = maxfx > sfx? maxfx : sfx;
-								pos = b + 1, ev &= ev - 1;
-							}
-							if (nb > pos) { sfx += (int64_t)(nb - pos) * afx; maxfx = maxfx > sfx? maxfx : sfx; }
+		// The reference's running score (align.c:266-297) is a double; here it is an integer in units of 2^-32, which is exact. With
+		// int8_t q and e, mmx_log2(1+len) is a float in [1,33) and so a multiple of 2^-23; q + e * mmx_log2(1+len) is then an exact
+		// double, a multiple of 2^-23 below 2^13 in magnitude, and times 2^32 an integer below 2^45 (tests/test_tail_penalty_exact.py).
+		int64_t matfx[25];
+		for (int i = 0; i < 25; ++i) matfx[i] = (int64_t)mat[i] << 32;
+		int64_t sfx = 0, maxfx = 0;
+		const int64_t afx = matfx[0];
+		const bool diag_ok = mat[0] > 0 && mat[6] == mat[0] && mat[12] == mat[0] && mat[18] == mat[0]; // one positive match score
+		int32_t blen = 0, mlen = 0, n_ambi_tot = 0, is_spliced = 0;
+		for (uint32_t k = 0; k < p->n_cigar; ++k) {
+			uint32_t op = p->cigar[k] & 0xf, len = p->cigar[k] >> 4;
+			if (op == MM_CIGAR_MATCH) {
+				int n_ambi = 0, n_diff = 0;
+				const uint8_t *pq = qseq + qoff, *pt = tseq + toff;
+				if (diag_ok) {
+					// runs of identical unambiguous bases add run * a at once (the running score only rises there, so
+					// testing the maximum at the end of the run is the same as testing it at every base); 16 bases
+					// per comparison, both buffers carry 16 bytes of slack
+					for (uint32_t l0 = 0; l0 < len; l0 += 16) {
+						const uint32_t nb = len - l0 < 16? len - l0 : 16;
+						const __m128i vq = _mm_loadu_si128((const __m128i*)(pq + l0)), vt = _mm_loadu_si128((const __m128i*)(pt + l0));
+						const __m128i same = _mm_cmpeq_epi8(vq, vt), amb = _mm_cmpgt_epi8(_mm_or_si128(vq, vt), _mm_set1_epi8(3));
+						uint32_t ev = (uint32_t)_mm_movemask_epi8(_mm_or_si128(amb, _mm_xor_si128(same, _mm_set1_epi8(-1)))) & ((1u << nb) - 1);
+						uint32_t pos = 0;
+						while (ev) {
+							const uint32_t b = (uint32_t)__builtin_ctz(ev);
+							if (b > pos) { sfx += (int64_t)(b - pos) * afx; maxfx = maxfx > sfx? maxfx : sfx; }
+							const int cq = pq[l0 + b], ct = pt[l0 + b];
+							if ((ct | cq) > 3) ++n_ambi; else ++n_diff;
+							sfx += matfx[ct * 5 + cq];
+							if (sfx < 0) sfx = 0;
+							else maxfx = maxfx > sfx? maxfx : sfx;
+							pos = b + 1, ev &= ev - 1;
 						}
-					} else
-					for (uint32_t l = 0; l < len; ++l) {
-						const int cq = pq[l], ct = pt[l];
-						const int amb = (ct | cq) > 3;
-						n_ambi += amb, n_diff += (ct != cq) & !amb;
-						sfx += matfx[ct * 5 + cq];
-						if (sfx < 0) sfx = 0;
-						else maxfx = maxfx > sfx? maxfx : sfx;
+						if (nb > pos) { sfx += (int64_t)(nb - pos) * afx; maxfx = maxfx > sfx? maxfx : sfx; }
 					}
-					blen += len - n_ambi, mlen += len - (n_ambi + n_diff), n_ambi_tot += n_ambi;
-					toff += len, qoff += len;
-				} else if (op == MM_CIGAR_INS || op == MM_CIGAR_DEL) {
-					int n_ambi = 0;
-					const uint8_t *sq = op == MM_CIGAR_INS? qseq + qoff : tseq + toff;
-					for (uint32_t l = 0; l < len; ++l) if (sq[l] > 3) ++n_ambi;
-					blen += len - n_ambi, n_ambi_tot += n_ambi;
-					const double pen = log_gap? q + (double)e * mmx_log2(1.0 + len) : (double)(q + e);
-					const double scaled = pen * 4294967296.0;
-					const int64_t pfx = (int64_t)scaled;
-					if ((double)pfx != scaled || pen > 1e6 || pen < -1e6) { fixed_ok = false; break; }
-					sfx -= pfx;
+				} else
+				for (uint32_t l = 0; l < len; ++l) {
+					const int cq = pq[l], ct = pt[l];
+					const int amb = (ct | cq) > 3;
+					n_ambi += amb, n_diff += (ct != cq) & !amb;
+					sfx += matfx[ct * 5 + cq];
 					if (sfx < 0) sfx = 0;
-					if (op == MM_CIGAR_INS) qoff += len; else toff += len;
-				} else if (op == MM_CIGAR_N_SKIP) is_spliced = 1, toff += len;
-			}
-			if (fixed_ok) {
-				r->blen = blen, r->mlen = mlen, r->is_spliced = is_spliced, p->n_ambi += n_ambi_tot;
-				max = (double)maxfx / 4294967296.0;
-			}
+					else maxfx = maxfx > sfx? maxfx : sfx;
+				}
+				blen += len - n_ambi, mlen += len - (n_ambi + n_diff), n_ambi_tot += n_ambi;
+				toff += len, qoff += len;
+			} else if (op == MM_CIGAR_INS || op == MM_CIGAR_DEL) {
+				int n_ambi = 0;
+				const uint8_t *sq = op == MM_CIGAR_INS? qseq + qoff : tseq + toff;
+				for (uint32_t l = 0; l < len; ++l) if (sq[l] > 3) ++n_ambi;
+				blen += len - n_ambi, n_ambi_tot += n_ambi;
+				const double pen = log_gap? q + (double)e * mmx_log2(1.0 + len) : (double)(q + e);
+				sfx -= (int64_t)(pen * 4294967296.0);
+				if (sfx < 0) sfx = 0;
+				if (op == MM_CIGAR_INS) qoff += len; else toff += len;
+			} else if (op == MM_CIGAR_N_SKIP) is_spliced = 1, toff += len;
 		}
-		if (!fixed_ok) { // the reference's loop as written (align.c:266-297)
-			toff = qoff = 0, s = 0.0, max = 0.0;
-			r->blen = r->mlen = 0, r->is_spliced = 0;
-			for (uint32_t k = 0; k < p->n_cigar; ++k) {
-				uint32_t op = p->cigar[k] & 0xf, len = p->cigar[k] >> 4;
-				if (op == MM_CIGAR_MATCH) {
-					int n_ambi = 0, n_diff = 0;
-					for (uint32_t l = 0; l < len; ++l) {
-						int cq = qseq[qoff + l], ct = tseq[toff + l];
-						if (ct > 3 || cq > 3) ++n_ambi;
-						else if (ct != cq) ++n_diff;
-						s += mat[ct * 5 + cq];
-						if (s < 0) s = 0;
-						else max = max > s? max : s;
-					}
-					r->blen += len - n_ambi, r->mlen += len - (n_ambi + n_diff), p->n_ambi += n_ambi;
-					toff += len, qoff += len;
-				} else if (op == MM_CIGAR_INS || op == MM_CIGAR_DEL) {
-					int n_ambi = 0;
-					const uint8_t *sq = op == MM_CIGAR_INS? qseq + qoff : tseq + toff;
-					for (uint32_t l = 0; l < len; ++l) if (sq[l] > 3) ++n_ambi;
-					r->blen += len - n_ambi, p->n_ambi += n_ambi;
-					if (log_gap) s -= q + (double)e * mmx_log2(1.0 + len);
-					else s -= q + e;
-					if (s < 0) s = 0;
-					if (op == MM_CIGAR_INS) qoff += len; else toff += len;
-				} else if (op == MM_CIGAR_N_SKIP) r->is_spliced = 1, toff += len;
-			}
-		}
-		p->dp_max = p->dp_max0 = (int32_t)(max + .499);
+		r->blen = blen, r->mlen = mlen, r->is_spliced = is_spliced, p->n_ambi += n_ambi_tot;
+		p->dp_max = p->dp_max0 = (int32_t)((double)maxfx / 4294967296.0 + .499);
 		assert(qoff == r->qe - r->qs && toff == r->re - r->rs);
 		if (is_eqx) update_cigar_eqx(r, qseq, tseq);
 	}

@@ -5,9 +5,10 @@
 // every aligned base in mm_update_extra (align.c:254-303) for blen / mlen / n_ambi / dp_max. On the host that was the largest single
 // cost of the replay driver (a third of its CPU time: one pass over every aligned base of every read). Here one warp per hit does
 // the three steps straight from the job CIGARs that are still in the device arena, so only the final CIGAR and eight integers per
-// hit cross PCIe. The running score of mm_update_extra is a sum of integers and of e * mg_log2(1+len) terms that are exact
-// multiples of 2^-32 (float mantissa), so it is carried in 2^-32 fixed point -- exactly the reference's double arithmetic; a hit
-// whose penalty is not representable is flagged (status 1) and redone by the host driver.
+// hit cross PCIe. The running score of mm_update_extra is a sum of integers and of q + e * mg_log2(1+len) gap penalties that are
+// exact multiples of 2^-23 for int8_t q and e (see update_extra in align.cc), so it is carried in 2^-32 fixed point -- exactly the
+// reference's double arithmetic. A hit whose CIGAR does not consume its query and target spans, which the reference asserts, is
+// flagged (status 2) and redone by the host driver.
 #include "pipeline.h"
 
 namespace {
@@ -225,10 +226,7 @@ __global__ void __launch_bounds__(128) finalize_kernel(const FinReg *regs, const
 			else { for (int i = 0; i < len; ++i) if (A.t(toff + i) > 3) ++amb; }
 			blen += len - amb, n_ambi += amb;
 			const double pen = par.log_gap? par.q + (double)par.e * mmx_log2((float)(1.0 + len)) : (double)(par.q + par.e);
-			const double scaled = pen * 4294967296.0;
-			const long long pfx = (long long)scaled;
-			if ((double)pfx != scaled || pen > 1e6 || pen < -1e6) status = 1;
-			walk_step(wk, -pfx);
+			walk_step(wk, -(long long)(pen * 4294967296.0));
 		} else if (valid && op == MM_CIGAR_N_SKIP) spliced = 1;
 		#pragma unroll
 		for (int o = 1; o < 32; o <<= 1) { // ordered reduction: lane 0 ends with the chunk's stretch
@@ -245,9 +243,9 @@ __global__ void __launch_bounds__(128) finalize_kernel(const FinReg *regs, const
 	#pragma unroll
 	for (int o = 16; o > 0; o >>= 1) {
 		blen += __shfl_xor_sync(full, blen, o), mlen += __shfl_xor_sync(full, mlen, o), n_ambi += __shfl_xor_sync(full, n_ambi, o);
-		spliced |= __shfl_xor_sync(full, spliced, o), status |= (__shfl_xor_sync(full, status, o) & 1);
+		spliced |= __shfl_xor_sync(full, spliced, o);
 	}
-	if (nc > 0 && (carry_q + qshift != R.qspan || carry_t + tshift != R.tspan) && status == 0) status = 2;
+	if (nc > 0 && (carry_q + qshift != R.qspan || carry_t + tshift != R.tspan)) status = 2;
 	if (lane == 0) {
 		FinOut o;
 		o.n_cigar = (int32_t)nc, o.blen = blen, o.mlen = mlen, o.n_ambi = n_ambi, o.qshift = qshift, o.tshift = tshift, o.status = status, o.is_spliced = spliced;

@@ -31,6 +31,7 @@ double hl_event_identity(const mm_reg1_t *r);
 void hl_update_dp_max(int qlen, int n_regs, mm_reg1_t *regs, float frac, int a, int b);
 
 // ---- align.cc: the alignment driver (mm_align_skeleton / mm_align1, align.c:645-1120) as a replayable routine ----
+void hl_gen_mat(int8_t *mat, const mm_mapopt_t *opt); // the 5x5 score matrix of the options (align.c:11-38): the driver's and the kernels'
 struct KswKey {
 	int64_t q_start, t_start;
 	int32_t q_step, t_step, qlen, tlen, w, zdrop, end_bonus, flag;

@@ -621,19 +621,11 @@ static void chains_to_hits(Batch &b, const MapPass &pass)
 	b.lap("stage2 qseq encode");
 }
 
-// the ksw2 scoring of the options: align.c:11-38 via a throw-away driver-compatible matrix
+// the ksw2 scoring of the options, with the alignment driver's matrix
 static mmb_ksw_score_t ksw_score(const mm_mapopt_t *opt)
 {
 	mmb_ksw_score_t sc;
-	const int m = 5;
-	int8_t aa = (int8_t)(opt->a < 0? -opt->a : opt->a), bb2 = (int8_t)(opt->b > 0? -opt->b : opt->b);
-	int8_t sa = (int8_t)(opt->sc_ambi > 0? -opt->sc_ambi : opt->sc_ambi);
-	for (int i = 0; i < m - 1; ++i) { for (int k = 0; k < m - 1; ++k) sc.mat[i * m + k] = i == k? aa : bb2; sc.mat[i * m + m - 1] = sa; }
-	for (int k = 0; k < m; ++k) sc.mat[(m - 1) * m + k] = sa;
-	if (!(opt->transition == 0 || opt->transition == opt->b)) {
-		int8_t t = (int8_t)(opt->transition > 0? -opt->transition : opt->transition);
-		sc.mat[0 * m + 2] = t, sc.mat[1 * m + 3] = t, sc.mat[2 * m + 0] = t, sc.mat[3 * m + 1] = t;
-	}
+	hl_gen_mat(sc.mat, opt);
 	sc.q = (int8_t)opt->q, sc.e = (int8_t)opt->e, sc.q2 = (int8_t)opt->q2, sc.e2 = (int8_t)opt->e2;
 	sc.noncan = (int8_t)opt->noncan, sc.junc_bonus = (int8_t)opt->junc_bonus, sc.junc_pen = (int8_t)opt->junc_pen;
 	// mm_test_zdrop only compares the largest drop with zdrop and (unless the inversion probe is off, align.c:92) zdrop_inv: a
@@ -741,7 +733,7 @@ static void device_tail(Batch &b, const std::vector<int> &active, const FinPar &
 		bool ok;
 		{ HpScope hp_(HP_EXTRA); ok = hl_align_apply_fin(ra, n_regs, regs, h_fin + hoff[t], cp.data()); }
 		if (ok) hl_align_finish(b.opt, ra, &n_regs, regs);
-		else { // a gap penalty outside the fixed-point range (never with sane scoring): the host driver redoes the read
+		else { // a hit's CIGAR did not consume its query / target span (the reference asserts this): the host driver redoes the read
 			drop_regs(n_regs, regs);
 			regs = replay_read(b, r, false, &n_regs);
 			if (ra.incomplete) { fprintf(stderr, "[ERROR] minimap2_b200: host redo of a finished read is incomplete\n"); abort(); }

@@ -59,7 +59,7 @@ struct FinReg {
 	int32_t job_first, n_jobs;
 	int32_t pad;
 };
-struct FinOut { int32_t n_cigar, blen, mlen, n_ambi, dp_max, qshift, tshift, status, is_spliced, pad[3]; }; // status 0: done; else the host driver redoes the read
+struct FinOut { int32_t n_cigar, blen, mlen, n_ambi, dp_max, qshift, tshift, status, is_spliced, pad[3]; }; // status 0: done; 2: the CIGAR does not consume qspan / tspan, the host driver redoes the read
 struct FinPar { int8_t mat[25]; int8_t q, e, log_gap; };
 void mmb_finalize_device(mmb_ctx_t *ctx, const FinReg *d_regs, const FinJobRef *d_jobs, int n_regs, const uint8_t *d_query, const uint32_t *d_S,
 						 uint32_t *d_out, FinOut *d_res, const FinPar &par);
