@@ -437,30 +437,28 @@ __global__ void __launch_bounds__(64) chain_rescue_kernel(ChainArgs A, RescuePar
 	A.n_u[rd] = n_u, A.n_v[rd] = n_v;
 }
 
-__global__ void stk_len_kernel(const int64_t *a_off, int n_reads, int64_t *stk_off)
-{
-	int i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i < n_reads) stk_off[i] = mmx_rs_stack_len(a_off[i + 1] - a_off[i]);
-}
-
 } // namespace
 
 #include "scan.cuh"
 
-// scratch layout shared by the DP, backtrack and RMQ kernels: f,p,v,t (4 x int32 n_tot) | z (m128 n_tot) | b (m128 n_tot); sort stacks
+// Scratch of the DP, backtrack and RMQ kernels: f, p, v, t (4 x int32) | z (m128) | b (m128), n_tot+4 entries each, in scratch
+// (reserved here when `reserve`), and the per-read sort stacks that mmb_sort_stacks_async laid out in scratch2. The chainers reserve
+// the scratch; the rescue that follows them reuses it as it is.
+static void chain_scratch_layout(ChainArgs &A, int n_reads, int64_t n_tot, DevBuf &scratch, DevBuf &scratch2, bool reserve)
+{
+	const size_t n = (size_t)n_tot + 4;
+	uint8_t *s = (uint8_t*)(reserve? scratch.reserve(n * (16 + 16 + 16) + 256) : scratch.p);
+	A.f = (int32_t*)s, A.p = A.f + n, A.v = A.p + n, A.t = A.v + n;
+	A.z = (m128*)(s + n * 16), A.b = A.z + n;
+	A.stk_off = (int64_t*)scratch2.p, A.stk = mmb_sort_stacks((int64_t*)scratch2.p, n_reads);
+}
+
 static void chain_scratch_setup(mmb_ctx_t *ctx, ChainArgs &A, int n_reads, const m128 *d_a, const int64_t *d_a_off, int64_t n_tot,
 								int32_t *d_n_u, int32_t *d_n_v, uint64_t *d_u, m128 *d_a_out, DevBuf &scratch, DevBuf &scratch2)
 {
 	A.n_reads = n_reads, A.a_off = d_a_off, A.a = d_a;
-	const size_t n = (size_t)n_tot + 4;
-	uint8_t *s = (uint8_t*)scratch.reserve(n * (16 + 16 + 16) + 256);
-	A.f = (int32_t*)s, A.p = A.f + n, A.v = A.p + n, A.t = A.v + n;
-	A.z = (m128*)(s + n * 16), A.b = A.z + n;
-	int64_t *d_stk_off = (int64_t*)scratch2.reserve(((size_t)n_reads + 1) * 8 + ((size_t)n_tot / 65 * 24 + (size_t)n_reads * 48 + 64) * 4);
-	stk_len_kernel<<<(n_reads + 255) / 256, 256, 0, ctx->stream>>>(d_a_off, n_reads, d_stk_off);
-	++ctx->n_launch;
-	mmb_exclusive_scan_i64_async(ctx, d_stk_off, n_reads);
-	A.stk_off = d_stk_off, A.stk = (int32_t*)(d_stk_off + n_reads + 1);
+	mmb_sort_stacks_async(ctx, d_a_off, n_reads, n_tot, scratch2, 0);
+	chain_scratch_layout(A, n_reads, n_tot, scratch, scratch2, true);
 	A.n_u = d_n_u, A.n_v = d_n_v, A.u = d_u, A.a_out = d_a_out;
 }
 
@@ -514,12 +512,7 @@ void mmb_chain_rescue_device(mmb_ctx_t *ctx, const RescuePar *rp, int n_reads, c
 	ChainArgs A;
 	memset(&A, 0, sizeof(A));
 	A.n_reads = n_reads, A.a_off = d_a_off, A.a = nullptr;
-	const size_t n = (size_t)n_tot + 4;
-	uint8_t *s = (uint8_t*)scratch.p;
-	A.f = (int32_t*)s, A.p = A.f + n, A.v = A.p + n, A.t = A.v + n;
-	A.z = (m128*)(s + n * 16), A.b = A.z + n;
-	int64_t *d_stk_off = (int64_t*)scratch2.p;
-	A.stk_off = d_stk_off, A.stk = (int32_t*)(d_stk_off + n_reads + 1);
+	chain_scratch_layout(A, n_reads, n_tot, scratch, scratch2, false);
 	A.n_u = d_n_u, A.n_v = d_n_v, A.u = d_u, A.a_out = d_a_out;
 	RescuePar R = *rp;
 	R.tree = (uint8_t*)treebuf.reserve(((size_t)tot_v + (size_t)n_reads + 8) * 64);

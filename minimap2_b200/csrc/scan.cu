@@ -1,5 +1,6 @@
 // minimap2_b200/csrc/scan.cu -- three-phase exclusive scan (tile sums -> scan of sums -> add), int64.
 #include "scan.cuh"
+#include "mm_algo.cuh"
 
 namespace {
 const int TILE = 2048;      // elements per CTA (256 threads x 8)
@@ -55,6 +56,12 @@ __global__ void __launch_bounds__(256) scan_sums_kernel(int64_t *tile_sum, int64
 	}
 	if (threadIdx.x == 0 && d) d[n] = carry;
 }
+
+__global__ void stk_len_kernel(const int64_t *a_off, int n_reads, int64_t *stk_off)
+{
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n_reads) stk_off[i] = mmx_rs_stack_len(a_off[i + 1] - a_off[i]);
+}
 } // namespace
 
 void mmb_exclusive_scan_i64_async(mmb_ctx_t *ctx, int64_t *d, int64_t n)
@@ -68,6 +75,16 @@ void mmb_exclusive_scan_i64_async(mmb_ctx_t *ctx, int64_t *d, int64_t n)
 	scan_tile_kernel<<<(unsigned)n_tiles, 256, 0, ctx->stream>>>(d, n, ts, 1);
 	MMB_CUDA_CHECK(cudaGetLastError());
 	ctx->n_launch += 3;
+}
+
+int64_t *mmb_sort_stacks_async(mmb_ctx_t *ctx, const int64_t *a_off, int n_reads, int64_t n_tot, DevBuf &buf, size_t head_bytes)
+{
+	const size_t n_stk = (size_t)n_tot / 65 * 24 + (size_t)n_reads * 48 + 64; // >= the sum of mmx_rs_stack_len over the reads
+	int64_t *stk_off = (int64_t*)((uint8_t*)buf.reserve(head_bytes + ((size_t)n_reads + 1) * 8 + n_stk * 4) + head_bytes);
+	stk_len_kernel<<<(n_reads + 255) / 256, 256, 0, ctx->stream>>>(a_off, n_reads, stk_off);
+	++ctx->n_launch;
+	mmb_exclusive_scan_i64_async(ctx, stk_off, n_reads);
+	return stk_off;
 }
 
 int64_t mmb_exclusive_scan_i64(mmb_ctx_t *ctx, int64_t *d, int64_t n, bool with_total)

@@ -44,7 +44,7 @@ def check_case(L, ctx, contigs, reads, w=10, k=15, flag=0, mid_occ=10, q_occ_fra
     reads = [bytes(r) for r in reads]
     got = device_seeds(L, ctx, mi, reads, flag, mid_occ, q_occ_frac, max_max_occ, occ_dist)
     idx = O.OracleIndex(seqs, names, w, k)
-    stats = dict(anchors=0, ties=0, big=0)
+    stats = dict(anchors=0, ties=0, big=0, wide=0)
     for i, s in enumerate(reads):
         ea, erep, emp = idx.anchors(s, flag=flag, mid_occ=mid_occ, q_occ_frac=q_occ_frac, max_max_occ=max_max_occ, occ_dist=occ_dist) if len(s) else (np.zeros((0, 2), dtype=np.uint64), 0, np.zeros(0, dtype=np.uint64))
         ga, grep_, gmp = got[i]
@@ -53,12 +53,25 @@ def check_case(L, ctx, contigs, reads, w=10, k=15, flag=0, mid_occ=10, q_occ_fra
         assert ga.shape == ea.shape, (i, ga.shape, ea.shape)
         assert (ga == ea).all(), (i, int(np.argmax((ga != ea).any(axis=1))))
         stats["anchors"] += len(ea)
+        if len(ga):  # sort keys that differ in more than 33 bit positions: the radix kernels leave such reads to sort_block_kernel
+            stats["wide"] += int(bin(int(np.bitwise_or.reduce(ga[:, 0] ^ ga[0, 0]))).count("1") > 33)
         if len(ea) > 64:
             stats["big"] += 1
             stats["ties"] += int((ea[1:, 0] == ea[:-1, 0]).any())
     idx.close()
     L.mm_idx_destroy(mi)
     return stats
+
+
+def n_minimizers(seq, w, k, q_occ_max, q_occ_frac):
+    """minimizers of a read after the query-side filter (mm_seed_mz_flt, seed.c:5-28), from the oracle's sketch"""
+    x = O.oracle_sketch(bytes(seq), w, k)[:, 0]
+    n = len(x)
+    if n <= q_occ_max or q_occ_frac <= 0 or q_occ_max <= 0:
+        return n
+    _, inv, cnt = np.unique(x, return_inverse=True, return_counts=True)
+    c = cnt[inv]
+    return int((~(((c > q_occ_max) & (c > np.float32(n) * np.float32(q_occ_frac))) | (x == 0))).sum())
 
 
 def repeat_rich_case(seed, glen, n_reads, rlen, rep=0.4, n_contigs=2):

@@ -1,5 +1,5 @@
-"""CPU: the seeding-stage kernels (mzflt / lookup / select_warp / select / expand / sort_radix / sort_exact_*), unmodified CUDA sources under
-the SIMT emulator, against the oracle (see tests/seed_check.py)."""
+"""CPU: the seeding-stage kernels (mzflt / lookup / select / expand / sort_radix / sort_exact_*), unmodified CUDA sources under the SIMT
+emulator, against the oracle (see tests/seed_check.py)."""
 import ctypes as C
 import os
 import sys
@@ -34,3 +34,13 @@ def test_emulated_seed_stage_sort_ties(emu):
     contigs, reads = SC.repeat_rich_case(8, 30_000, 3, 2500, rep=0.8, n_contigs=1)
     st = SC.check_case(L, ctx, contigs, reads, mid_occ=50, max_max_occ=400, occ_dist=50)
     assert st["ties"] >= 1
+
+
+def test_emulated_seed_stage_long_reads(emu):
+    """reads with more than SEL_CAP (2048) minimizers after the query-side filter: select_kernel keeps their seeds in global memory"""
+    L, ctx = emu
+    contigs, reads = SC.repeat_rich_case(4, 60_000, 4, 8000, rep=0.5)
+    cfg = dict(w=5, mid_occ=8, q_occ_frac=0.01)
+    assert max(SC.n_minimizers(r, cfg["w"], 15, cfg["mid_occ"], cfg["q_occ_frac"]) for r in reads) > 2048
+    st = SC.check_case(L, ctx, contigs, reads, **cfg)
+    assert st["anchors"] > 500 and st["big"] >= 3

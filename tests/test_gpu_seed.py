@@ -2,8 +2,10 @@
 skip_seed's strand rule, anchor expansion, anchor sort incl. the reference's unstable tie order) through mmb_seed_batch_host against the
 oracle restatement (oracle/mm2o_seed.c). See tests/seed_check.py."""
 import ctypes as C
+import numpy as np
 import pytest
 import seed_check as SC
+import synth
 
 pytestmark = pytest.mark.gpu
 
@@ -36,3 +38,16 @@ def test_seed_stage_sort_ties_and_size_classes(dev):
     reads += [r[:n] for r, n in zip(reads[:12], (200, 500, 900, 1500, 2500, 3500, 5000, 7000, 9000, 10000, 11000, 11500))]
     st = SC.check_case(L, ctx, contigs, reads, mid_occ=60, max_max_occ=600, occ_dist=100)
     assert st["ties"] >= 5
+
+
+def test_seed_stage_wide_keys(dev):
+    """sort keys that differ in more than 33 bit positions, as on a human reference: the radix kernels hand these reads to
+    sort_block_kernel, and the ones with equal keys on to the exact emulation. 64 contigs give 6 contig bits; the last one holds a
+    reverse-complemented copy of chr0 at 2^27 - 2^14 after N padding, so positions differ in bits 0-26, plus the strand bit."""
+    L, ctx = dev
+    contigs = synth.random_genome(640_000, 13, n_contigs=63, repeat_frac=0.3)
+    seg = contigs[0]
+    contigs.append(np.concatenate([np.full((1 << 27) - (1 << 14), ord("N"), dtype=np.uint8), synth.revcomp(seg)]))
+    reads = synth.make_reads([seg], 40, 4000, 0.08, 63) + [bytes(seg[1000:9000]) * 2]  # the tandem read has equal keys
+    st = SC.check_case(L, ctx, contigs, reads, mid_occ=20)
+    assert st["wide"] >= 40 and st["ties"] >= 1
