@@ -706,10 +706,10 @@ void mmb_ksw_fast_plan(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, const std::vec
 					   const uint8_t *d_query, const void *d_target, int t_packed, mmb_ksw_res_t *d_res, uint32_t *d_cigar, int64_t cigar_cap,
 					   unsigned long long *d_cigar_used, int *d_order_all, std::vector<KswPlan> &plans);
 
-// Host-side tiering + launch. Tiers by max(qlen,tlen): warp-per-job for <=1024, CTA-per-job above.
-void mmb_ksw_launch(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, int n_jobs, const mmb_ksw_job_t *h_jobs, const mmb_ksw_job_t *d_jobs,
-					const uint8_t *d_query, const void *d_target, int t_packed,
-					mmb_ksw_res_t *d_res, uint32_t *d_cigar, int64_t cigar_cap, unsigned long long *d_cigar_used)
+// Host-side tiering. Tiers by max(qlen,tlen): warp-per-job for <=1024, CTA-per-job above. Nothing goes on the stream.
+void mmb_ksw_plan(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, int n_jobs, const mmb_ksw_job_t *h_jobs, const mmb_ksw_job_t *d_jobs,
+				  const uint8_t *d_query, const void *d_target, int t_packed,
+				  mmb_ksw_res_t *d_res, uint32_t *d_cigar, int64_t cigar_cap, unsigned long long *d_cigar_used, KswLaunch &K)
 {
 	if (n_jobs <= 0) return;
 	KswArgs A;
@@ -785,20 +785,23 @@ void mmb_ksw_launch(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, int n_jobs, const
 		int groups = std::min((int)llj.size(), ctx->n_sm * 16 * 4);
 		int grid = (groups * 8 + 127) / 128;
 		groups = grid * 16;
-		L.ws = (int16_t*)ctx->d_e.reserve(L.ws_stride * (size_t)groups);
 		int *d_order = (int*)ctx->d_g.reserve(((size_t)n_jobs * 3 + 256) * sizeof(int)) + (size_t)n_jobs * 2 + 128;
-		MMB_CUDA_CHECK(cudaMemcpyAsync(d_order + 1, llj.data(), llj.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-		MMB_CUDA_CHECK(cudaMemsetAsync(d_order, 0, sizeof(int), ctx->stream));
 		L.counter = d_order, L.order = d_order + 1;
-		ProfScope prof(ctx, MMB_PROF_OTHER, 0);
-		ksw_ll_kernel<<<grid, 128, 0, ctx->stream>>>(L);
-		MMB_CUDA_CHECK(cudaGetLastError());
-		++ctx->n_launch;
+		K.ll.pws_bytes = L.ws_stride * (size_t)groups; // the probes' workspace is the traceback workspace of the kernels after them
+		K.ll.order = std::move(llj), K.ll.d_order = d_order;
+		K.ll.go = [=](uint8_t *ws, uint32_t *) {
+			LLArgs B = L;
+			B.ws = (int16_t*)ws;
+			ksw_ll_kernel<<<grid, 128, 0, ctx->stream>>>(B);
+			MMB_CUDA_CHECK(cudaGetLastError());
+			++ctx->n_launch;
+		};
 	}
 	if (ctx->profiling) ctx->prof_bytes[MMB_PROF_KSW] += io_bytes + cells; // reference-layout algorithmic bytes: sequences + 1 B/cell traceback (+4 B per CIGAR op, added by the caller)
 	int *d_queues = (int*)ctx->d_g.reserve(((size_t)n_jobs * 3 + 256) * sizeof(int)); // queues: [0,n+64) fast path | [n+64,2n+128) universal tiers | [2n+128,..) ll
 	size_t g_off = (size_t)n_jobs + 64;
-	std::vector<KswPlan> plans;
+	std::vector<KswPlan> &plans = K.plans;
+	K.cells = cells;
 	mmb_ksw_fast_plan(ctx, sc, fastj, h_jobs, d_jobs, d_query, d_target, t_packed, d_res, d_cigar, cigar_cap, d_cigar_used, d_queues, plans);
 	for (int pass = 0; pass < 2; ++pass) { // 0: dual-affine (ksw_extd2), 1: spliced (ksw_exts2)
 		if (pass == 1) { // ksw2_exts2_sse.c:71-95: no (q,e)/(q2,e2) reordering; the intron state has no extension cost
@@ -851,10 +854,9 @@ void mmb_ksw_launch(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, int n_jobs, const
 		while ((size_t)grid * nw * (maxp + gws_stride) > ((size_t)2 << 30) && grid > 1) grid = (grid + 1) / 2;
 		A.pws_stride = maxp, A.cigws_stride = (size_t)maxsum + 8;
 		int *d_order = d_queues + g_off; g_off += v.size() + 1;
-		MMB_CUDA_CHECK(cudaMemcpyAsync(d_order + 1, v.data(), v.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-		MMB_CUDA_CHECK(cudaMemsetAsync(d_order, 0, sizeof(int), ctx->stream));
 		A.counter = d_order, A.order = d_order + 1, A.n = (int)v.size();
 		KswPlan pl;
+		pl.order = std::move(v), pl.d_order = d_order;
 		const size_t pws_area = A.pws_stride * (size_t)grid * nw;
 		pl.pws_bytes = pws_area + gws_stride * (size_t)grid * nw, pl.cigws_bytes = A.cigws_stride * 4 * (size_t)grid * nw;
 		const KswArgs A0 = A;
@@ -869,11 +871,36 @@ void mmb_ksw_launch(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, int n_jobs, const
 		plans.push_back(pl);
 	}
 	}
-	// one workspace sized for the largest launch (they run one after another on the stream), then the kernels back to back
-	size_t pws_bytes = 0, cigws_bytes = 0;
-	for (const KswPlan &pl : plans) pws_bytes = std::max(pws_bytes, pl.pws_bytes), cigws_bytes = std::max(cigws_bytes, pl.cigws_bytes);
+}
+
+// The launch set on ctx->stream: the queue uploads, the probes, then the other kernels back to back in one workspace sized for the
+// largest launch (they run one after another on the stream).
+void mmb_ksw_enqueue(mmb_ctx_t *ctx, const KswLaunch &K)
+{
+	size_t pws_bytes = K.ll.pws_bytes, cigws_bytes = 0;
+	for (const KswPlan &pl : K.plans) pws_bytes = std::max(pws_bytes, pl.pws_bytes), cigws_bytes = std::max(cigws_bytes, pl.cigws_bytes);
 	uint8_t *pws = (uint8_t*)ctx->d_e.reserve(pws_bytes);
 	uint32_t *cigws = (uint32_t*)ctx->d_f.reserve(cigws_bytes);
-	ProfScope prof(ctx, MMB_PROF_KSW, cells);
-	for (const KswPlan &pl : plans) pl.go(pws, cigws);
+	auto upload = [&](const KswPlan &pl) {
+		MMB_CUDA_CHECK(cudaMemcpyAsync(pl.d_order + 1, pl.order.data(), pl.order.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+		MMB_CUDA_CHECK(cudaMemsetAsync(pl.d_order, 0, sizeof(int), ctx->stream));
+	};
+	if (K.ll.go) {
+		upload(K.ll);
+		ProfScope prof(ctx, MMB_PROF_OTHER, 0);
+		K.ll.go(pws, nullptr);
+	}
+	for (const KswPlan &pl : K.plans) upload(pl);
+	ProfScope prof(ctx, MMB_PROF_KSW, K.cells);
+	for (const KswPlan &pl : K.plans) pl.go(pws, cigws);
+}
+
+void mmb_ksw_launch(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, int n_jobs, const mmb_ksw_job_t *h_jobs, const mmb_ksw_job_t *d_jobs,
+					const uint8_t *d_query, const void *d_target, int t_packed,
+					mmb_ksw_res_t *d_res, uint32_t *d_cigar, int64_t cigar_cap, unsigned long long *d_cigar_used)
+{
+	if (n_jobs <= 0) return;
+	KswLaunch K;
+	mmb_ksw_plan(ctx, sc, n_jobs, h_jobs, d_jobs, d_query, d_target, t_packed, d_res, d_cigar, cigar_cap, d_cigar_used, K);
+	mmb_ksw_enqueue(ctx, K);
 }

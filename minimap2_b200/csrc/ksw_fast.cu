@@ -674,8 +674,8 @@ bool mmb_ksw_fast_eligible(const mmb_ksw_job_t &j)
 	return w >= std::max(j.qlen, j.tlen);
 }
 
-// Launches the fast kernel over the eligible jobs listed in `idx` (indices into the batch). Asynchronous on ctx->stream
-// except for the queue-order upload, which is synchronised before returning.
+// Plans the fast kernel's launches over the eligible jobs listed in `idx` (indices into the batch), one per width class. Host
+// work only: mmb_ksw_enqueue uploads the queues and launches.
 void mmb_ksw_fast_plan(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, const std::vector<int> &idx, const mmb_ksw_job_t *h_jobs, const mmb_ksw_job_t *d_jobs,
 					   const uint8_t *d_query, const void *d_target, int t_packed, mmb_ksw_res_t *d_res, uint32_t *d_cigar, int64_t cigar_cap,
 					   unsigned long long *d_cigar_used, int *d_order_all, std::vector<KswPlan> &plans)
@@ -746,10 +746,9 @@ void mmb_ksw_fast_plan(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, const std::vec
 		A.pws_stride = ((size_t)(maxq + 2 * LNW[k] + 2) * W + 255) & ~(size_t)255; // one row per step of the lane-skewed sweep
 		A.cigws_stride = (size_t)maxsum + 8;
 		int *d_order = d_order_all + order_off; order_off += v[k].size() + 1;
-		MMB_CUDA_CHECK(cudaMemcpyAsync(d_order + 1, v[k].data(), v[k].size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-		MMB_CUDA_CHECK(cudaMemsetAsync(d_order, 0, sizeof(int), ctx->stream));
 		A.counter = d_order, A.order = d_order + 1, A.n = (int)v[k].size();
 		KswPlan pl;
+		pl.order = std::move(v[k]), pl.d_order = d_order;
 		pl.pws_bytes = A.pws_stride * (size_t)grid * nwk * NJ + 256 /* the tile loads may read past the last row */, pl.cigws_bytes = A.cigws_stride * 4 * (size_t)grid * nwk * NJ;
 		const FastArgs A0 = A;
 		pl.go = [=](uint8_t *pws, uint32_t *cigws) {

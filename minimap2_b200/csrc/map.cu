@@ -11,9 +11,12 @@
 #include "pipeline.h"
 #include "hostlogic.h"
 #include "scan.cuh"
+#include "ksw_plan.h"
 #include "fastx.h"
 #include <thread>
 #include <unistd.h>
+#include <malloc.h>
+#include <climits>
 #include <atomic>
 #include <functional>
 #include <cstring>
@@ -26,10 +29,6 @@
 extern "C" double realtime(void);
 extern "C" double cputime(void);
 int mmb_resident_reads(void);
-
-void mmb_ksw_launch(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, int n_jobs, const mmb_ksw_job_t *h_jobs, const mmb_ksw_job_t *d_jobs,
-					const uint8_t *d_query, const void *d_target, int t_packed,
-					mmb_ksw_res_t *d_res, uint32_t *d_cigar, int64_t cigar_cap, unsigned long long *d_cigar_used);
 
 namespace {
 
@@ -107,9 +106,15 @@ void parallel_for(int64_t n, int n_threads, const std::function<void(int64_t, in
 	g_pool->run(n, fn);
 }
 
-int g_gpu_slots = getenv("MM_B200_GPU_SLOTS")? std::max(1, atoi(getenv("MM_B200_GPU_SLOTS"))) : 4;
+const int g_gpu_slots_env = getenv("MM_B200_GPU_SLOTS")? std::max(1, atoi(getenv("MM_B200_GPU_SLOTS"))) : 0;
+int g_gpu_slots = g_gpu_slots_env; // 0: two thirds of the groups of the batch
+int g_batch_groups = 1;
 // FIFO gate bounding how many groups are in a device phase at once: with more groups than slots, the groups fall out of
-// lock-step and one group's host phase overlaps the others' kernels.
+// lock-step and one group's host phase overlaps the others' kernels. By default two thirds of the groups may hold a slot (8 of
+// 12). A group in a device phase spends most of it waiting for its stream (mmb_stream_sync, which leaves the CPU to the host
+// phases), a map-ont group about twice as long as in its host phases; so with a third of the groups on the host the device is
+// rarely without work. Fewer slots keep groups waiting to enter stage 1 while the groups that got through run host phases
+// with the device idle; with one slot per group they all move through the pipeline in lock-step (DESIGN §6).
 class GpuGate {
 public:
 	// Two request classes: 0 = stage 1 of a group (sketch..chain), 1 = an alignment wave. Each class is FIFO. While both have
@@ -128,7 +133,7 @@ public:
 		cv_.notify_all();
 	}
 	void release(int cls) { std::lock_guard<std::mutex> lk(mu_); --in_[cls]; cv_.notify_all(); }
-	static int slots() { return g_gpu_slots; }
+	static int slots() { return g_gpu_slots > 0? g_gpu_slots : std::max(1, (2 * g_batch_groups + 2) / 3); }
 private:
 	std::mutex mu_;
 	std::condition_variable cv_;
@@ -137,10 +142,25 @@ private:
 };
 GpuGate g_gate;
 struct GateHold {
-	bool on; int cls;
-	GateHold(bool use, int cls_) : on(use), cls(cls_) { if (on) g_gate.acquire(cls); }
-	void drop() { if (on) g_gate.release(cls), on = false; }
+	mmb_ctx_t *ctx; bool use, on = false; int cls;
+	GateHold(mmb_ctx_t *c, bool use_, int cls_, bool now = true) : ctx(c), use(use_), cls(cls_) { if (now) take(); }
+	void take() {
+		if (!use || on) return;
+		mmb_tl(ctx, MMB_TL_GATE_REQ, cls);
+		g_gate.acquire(cls);
+		mmb_tl(ctx, MMB_TL_GATE_GRANT, cls);
+		on = true;
+	}
+	void drop() { if (on) g_gate.release(cls), mmb_tl(ctx, MMB_TL_GATE_REL, cls), on = false; }
 	~GateHold() { drop(); }
+};
+
+// Host phases of a group's batch on the scheduler timeline (MMB_TL_HOST_BEGIN / _END arguments)
+enum HostPhase { HPH_CONCAT, HPH_HITS, HPH_REPLAY, HPH_TAIL_PREP, HPH_TAIL_APPLY, HPH_JOBS, HPH_KSW_PLAN, HPH_SCATTER, HPH_FINALIZE };
+struct HostSpan {
+	mmb_ctx_t *ctx; int ph;
+	HostSpan(mmb_ctx_t *c, int p) : ctx(c), ph(p) { mmb_tl(ctx, MMB_TL_HOST_BEGIN, ph); }
+	~HostSpan() { mmb_tl(ctx, MMB_TL_HOST_END, ph); }
 };
 
 __global__ void encode_kernel(uint8_t *s, int64_t n)
@@ -249,7 +269,7 @@ struct BatchBufs { // device arenas reused across batches (per context)
 	PinBuf h_fin_in, h_fin_out;
 	DevBuf qlo, qhi, k_cnt;                // skip_seed inputs (ava / strand-restricted modes only)
 	DevBuf dreg, dreg_off;                 // masked intervals of the reads (-T / SDUST only)
-	PinBuf h_seq, h_misc, h_jobs, h_res;
+	PinBuf h_seq, h_misc, h_jobs, h_res, h_used;
 	std::vector<std::unique_ptr<PinBuf>> h_cig; // one CIGAR staging buffer per alignment wave (cached results point into them until the batch ends)
 	std::vector<ReadState> rs_pool;        // persistent per-read objects: their vectors keep capacity => no allocation in steady state
 	std::vector<ReadAlign> ra_pool;
@@ -275,7 +295,6 @@ bool supported_mode(const mm_idx_t *mi, const mm_mapopt_t *opt)
 
 } // namespace
 
-static double g_batch_t0 = 0;
 // pass: first mapping pass, or the re-chaining pass of map.c:293-316 over the reads the first pass left without a chain
 struct MapPass {
 	int occ_cut;        // max_occ argument of mm_collect_matches (map.c:174): mid_occ, or opt->max_occ when re-chaining
@@ -285,21 +304,6 @@ struct MapPass {
 
 namespace {
 
-// MM_B200_TIMING: wall time of each section of a group's batch, taken after a stream synchronise
-struct Lap {
-	mmb_ctx_t *ctx;
-	double t_last;
-	static bool on() { static const bool timing = getenv("MM_B200_TIMING") != nullptr; return timing; }
-	void operator()(const char *what)
-	{
-		if (!on()) return;
-		cudaStreamSynchronize(ctx->stream);
-		const double t = realtime();
-		fprintf(stderr, "[timing g%d] %-28s %.1f ms  @ %.1f - %.1f\n", ctx->group_id, what, 1e3 * (t - t_last), 1e3 * (t_last - g_batch_t0), 1e3 * (t - g_batch_t0));
-		t_last = t;
-	}
-};
-
 // One batch of a group on its way through the stages: what every stage reads, and what one stage hands to the next
 struct Batch {
 	mmb_ctx_t *ctx;
@@ -308,7 +312,6 @@ struct Batch {
 	const mm_idx_t *mi;
 	const mm_mapopt_t *opt;
 	int n_threads;
-	Lap lap;
 	std::vector<int> live;             // input indices of the reads that go through the pipeline (non-empty, within max_qlen)
 	std::vector<int64_t> off;          // n+1 offsets of the live reads back to back
 	int n = 0;
@@ -327,7 +330,7 @@ struct Batch {
 	size_t keep_used = 0;              // device CIGAR arenas (bb.cig_keep) handed out so far, counted across the waves of the batch
 	int wave = 0;
 	Batch(mmb_ctx_t *c, BatchBufs &b, bool g, const mm_idx_t *m, const mm_mapopt_t *o, int nt)
-		: ctx(c), bb(b), gated(g), mi(m), opt(o), n_threads(nt), lap{c, realtime()} {}
+		: ctx(c), bb(b), gated(g), mi(m), opt(o), n_threads(nt) {}
 };
 
 } // namespace
@@ -354,8 +357,9 @@ static bool take_reads(Batch &b, int n_reads, const int *qlens, const char **seq
 	return true;
 }
 
-// The reads to the device: host concat, H2D and nt4 encoding, the latter two skipped when the reads are resident (the group's
-// previous batch was the same reads). Returns the concatenated reads on the host (ASCII).
+// The reads to the device: host concat, H2D and nt4 encoding, all three skipped when the reads are resident (the group's previous
+// batch was the same reads) and nothing on the host needs them back to back. Returns the concatenated reads on the host (ASCII), or
+// null when they were not concatenated.
 static const uint8_t *upload_reads(GroupCtx &G, Batch &b)
 {
 	mmb_ctx_t *ctx = b.ctx;
@@ -365,15 +369,20 @@ static const uint8_t *upload_reads(GroupCtx &G, Batch &b)
 	const std::vector<int64_t> &off = b.off;
 	const int n = b.n;
 	const int64_t total_bases = b.total_bases;
-	uint8_t *h_seq = bb.h_seq.as<uint8_t>((size_t)total_bases + 16);
-	parallel_for(n, b.n_threads, [&](int64_t j, int) { memcpy(h_seq + off[j], rs[live[j]].seq, rs[live[j]].qlen); });
-	b.lap("host concat");
+	const bool resident_hit = mmb_resident_reads() && G.res_n == n && G.res_bases == total_bases && G.res_first == rs[live[0]].seq;
+	// in seeding only SDUST reads the host copy (seed_batch); 300 MB of memcpy per step is otherwise spent on the shared host pool
+	// while every group waits for it
+	uint8_t *h_seq = nullptr;
+	if (!resident_hit || b.opt->sdust_thres > 0) {
+		HostSpan hs_(ctx, HPH_CONCAT);
+		h_seq = bb.h_seq.as<uint8_t>((size_t)total_bases + 16);
+		parallel_for(n, b.n_threads, [&](int64_t j, int) { memcpy(h_seq + off[j], rs[live[j]].seq, rs[live[j]].qlen); });
+	}
 	uint8_t *d_seq = b.d_seq = bb.seq.as<uint8_t>((size_t)total_bases + 16);
 	int64_t *d_off = b.d_off = bb.off.as<int64_t>((size_t)n + 1);
 	int32_t *d_qlen = b.d_qlen = bb.qlen.as<int32_t>((size_t)n);
 	std::vector<int32_t> h_qlen(n);
 	for (int j = 0; j < n; ++j) h_qlen[j] = rs[live[j]].qlen;
-	const bool resident_hit = mmb_resident_reads() && G.res_n == n && G.res_bases == total_bases && G.res_first == rs[live[0]].seq;
 	ctx->last_d2h_bytes = 0, ctx->last_h2d_bytes = 0;
 	if (!resident_hit) {
 		MMB_CUDA_CHECK(cudaMemcpyAsync(d_seq, h_seq, total_bases, cudaMemcpyHostToDevice, ctx->stream));
@@ -429,7 +438,7 @@ static void seed_batch(Batch &b, const uint8_t *h_seq, const char **names, int o
 		MMB_CUDA_CHECK(cudaMemcpyAsync(d_dreg, flat.data(), sizeof(uint64_t) * flat.size(), cudaMemcpyHostToDevice, ctx->stream));
 		MMB_CUDA_CHECK(cudaMemcpyAsync(d_doff, doff.data(), sizeof(int64_t) * ((size_t)n + 1), cudaMemcpyHostToDevice, ctx->stream));
 		dust_filter_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(S.mz, d_mz_off, S.n_mz, d_dreg, d_doff, n);
-		MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream)); // the pageable staging vectors go out of scope here
+		mmb_stream_sync(ctx); // the pageable staging vectors go out of scope here
 		++ctx->n_launch;
 	}
 	if (opt->flag & (MM_F_NO_DIAG | MM_F_NO_DUAL | MM_F_FOR_ONLY | MM_F_REV_ONLY)) { // skip_seed (map.c:78-100) runs on the device
@@ -458,7 +467,7 @@ static void seed_batch(Batch &b, const uint8_t *h_seq, const char **names, int o
 			uint32_t *d_qlo = bb.qlo.as<uint32_t>((size_t)n), *d_qhi = bb.qhi.as<uint32_t>((size_t)n);
 			MMB_CUDA_CHECK(cudaMemcpyAsync(d_qlo, qlo.data(), sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
 			MMB_CUDA_CHECK(cudaMemcpyAsync(d_qhi, qhi.data(), sizeof(uint32_t) * n, cudaMemcpyHostToDevice, ctx->stream));
-			MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream)); // the host vectors go out of scope
+			mmb_stream_sync(ctx); // the host vectors go out of scope
 			S.name_rank = B->d_name_rank, S.q_name_lo = d_qlo, S.q_name_hi = d_qhi;
 		}
 	}
@@ -548,7 +557,8 @@ static void chain_batch(Batch &b, const MapPass &pass, GateHold &gate1)
 	MMB_CUDA_CHECK(cudaMemcpyAsync(h_du, d_du, sizeof(uint64_t) * (size_t)tot_u, cudaMemcpyDeviceToHost, ctx->stream));
 	MMB_CUDA_CHECK(cudaMemcpyAsync(h_dm, d_dm, sizeof(uint64_t) * (size_t)tot_m, cudaMemcpyDeviceToHost, ctx->stream));
 	MMB_CUDA_CHECK(cudaMemcpyAsync(h_rep, S.rep_len, sizeof(int32_t) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-	MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+	mmb_tl(ctx, MMB_TL_ENQUEUED, 0);
+	mmb_stream_sync(ctx);
 	gate1.drop();
 	ctx->last_d2h_bytes += misc_bytes;
 	if (ctx->profiling) {
@@ -572,6 +582,7 @@ static void chains_to_hits(Batch &b, const MapPass &pass)
 	const mm_mapopt_t *opt = b.opt;
 	const int n = b.n;
 	const bool with_cigar = (opt->flag & MM_F_CIGAR) != 0;
+	HostSpan hs_(b.ctx, HPH_HITS);
 	if (with_cigar && bb.qseq_pool.size() < (size_t)b.total_bases * 2 + 16) bb.qseq_pool.resize((size_t)b.total_bases * 2 + 16);
 	parallel_for(n, b.n_threads, [&](int64_t j, int) {
 		HpScope hp_(HP_HITS);
@@ -607,8 +618,6 @@ static void chains_to_hits(Batch &b, const MapPass &pass)
 			r.ra = ra;
 		} else r.done = true, r.n_regs = n_regs0, r.regs = regs0, r.regs0 = nullptr;
 	});
-
-	b.lap("stage2 host hits");
 	if (with_cigar) { // nt4 forward / reverse-complement copies of the reads (align.c:1056-1061): room is set aside, the copies are made on first use
 		for (int j = 0; j < n; ++j) {
 			ReadState &r = rs[live[j]];
@@ -618,7 +627,6 @@ static void chains_to_hits(Batch &b, const MapPass &pass)
 			r.ra->qseq[0] = q0, r.ra->qseq[1] = q0 + r.qlen;
 		}
 	}
-	b.lap("stage2 qseq encode");
 }
 
 // the ksw2 scoring of the options, with the alignment driver's matrix
@@ -680,6 +688,7 @@ static void device_tail(Batch &b, const std::vector<int> &active, const FinPar &
 	BatchBufs &bb = b.bb;
 	const mm_idx_t *mi = b.mi;
 	const size_t nf = fr.size();
+	mmb_tl(ctx, MMB_TL_HOST_BEGIN, HPH_TAIL_PREP);
 	std::vector<int64_t> hoff(nf + 1, 0), joff2(nf + 1, 0);
 	for (size_t t = 0; t < nf; ++t) {
 		const ReadAlign &ra = *rs[fr[t]].ra;
@@ -713,13 +722,15 @@ static void device_tail(Batch &b, const std::vector<int> &active, const FinPar &
 	const size_t out_bytes = sizeof(FinOut) * (size_t)n_hits + 4 * (size_t)tot_cig;
 	uint8_t *d_out = bb.fin_out.as<uint8_t>(out_bytes + 64);
 	uint8_t *h_out = bb.h_fin_out.as<uint8_t>(out_bytes + 64);
+	mmb_tl(ctx, MMB_TL_HOST_END, HPH_TAIL_PREP);
 	MMB_CUDA_CHECK(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
 	mmb_finalize_device(ctx, (const FinReg*)d_in, (const FinJobRef*)(d_in + sizeof(FinReg) * (size_t)n_hits), (int)n_hits, b.d_seq, (const uint32_t*)mi->B->d_S,
 						(uint32_t*)(d_out + sizeof(FinOut) * (size_t)n_hits), (FinOut*)d_out, fpar);
 	MMB_CUDA_CHECK(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-	MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+	mmb_tl(ctx, MMB_TL_ENQUEUED, 2);
+	mmb_stream_sync(ctx);
 	ctx->last_h2d_bytes += in_bytes, ctx->last_d2h_bytes += out_bytes;
-	b.lap("  device tail");
+	HostSpan hs2_(ctx, HPH_TAIL_APPLY);
 	const HlFinOut *h_fin = (const HlFinOut*)h_out;
 	const uint32_t *h_fcig = (const uint32_t*)(h_out + sizeof(FinOut) * (size_t)n_hits);
 	parallel_for((int64_t)nf, b.n_threads, [&](int64_t t, int) {
@@ -740,7 +751,6 @@ static void device_tail(Batch &b, const std::vector<int> &active, const FinPar &
 		}
 		post_align(b, r, n_regs, regs);
 	});
-	b.lap("  tail apply");
 }
 
 // One K3 wave: the ksw2 jobs the unfinished reads of the wave asked for run in chunks on the device, and the results are handed to
@@ -758,6 +768,7 @@ static int64_t ksw_wave(Batch &b, const std::vector<int> &active, const mmb_ksw_
 	}
 	const int64_t n_jobs = joff[active.size()];
 	if (n_jobs == 0) return 0;
+	mmb_tl(ctx, MMB_TL_HOST_BEGIN, HPH_JOBS);
 	// every wave executes all jobs the replays asked for, so each read advances by at least one ksw call per wave and the
 	// loop ends; reads that keep splitting under a very small z-drop (-z 30) legitimately need dozens of waves. The
 	// bound only guards against a logic error.
@@ -788,8 +799,9 @@ static int64_t ksw_wave(Batch &b, const std::vector<int> &active, const mmb_ksw_
 	for (int64_t i = 0; i < n_jobs; ++i) cap_tot += cig_est(jobs[i]);
 	while (bb.h_cig.size() <= (size_t)b.wave) bb.h_cig.emplace_back(new PinBuf);
 	uint32_t *h_cig = bb.h_cig[b.wave]->as<uint32_t>((size_t)cap_tot + 64);
-	GateHold gatew(b.gated, 1);
-	b.lap("  gate wait w");
+	mmb_tl(ctx, MMB_TL_HOST_END, HPH_JOBS);
+	// the slot is taken per chunk once its launch is planned: the host planning overlaps the other groups' kernels
+	GateHold gatew(ctx, b.gated, 1, false);
 	std::vector<int64_t> chunk_base; // offset of each chunk's CIGAR block inside h_cig
 	std::vector<const uint32_t*> chunk_dev; // and the block's address in its device arena
 	int64_t cig_fill = 0;
@@ -804,14 +816,23 @@ static int64_t ksw_wave(Batch &b, const std::vector<int> &active, const mmb_ksw_
 			while (bb.cig_keep.size() <= ki) bb.cig_keep.emplace_back(new DevBuf);
 			uint32_t *d_cig = bb.cig_keep[ki]->as<uint32_t>((size_t)cap + 4);
 			unsigned long long *d_used = (unsigned long long*)d_cig;
+			KswLaunch K;
+			{
+				HostSpan hs_(ctx, HPH_KSW_PLAN);
+				mmb_ksw_plan(ctx, &sc, (int)m, &jobs[c0], d_jobs, b.d_seq, b.mi->B->d_S, 1, d_res, d_cig + 2, cap, d_used, K);
+			}
+			gatew.take();
 			MMB_CUDA_CHECK(cudaMemcpyAsync(d_jobs, &jobs[c0], sizeof(mmb_ksw_job_t) * m, cudaMemcpyHostToDevice, ctx->stream));
 			MMB_CUDA_CHECK(cudaMemsetAsync(d_used, 0, 8, ctx->stream));
-			mmb_ksw_launch(ctx, &sc, (int)m, &jobs[c0], d_jobs, b.d_seq, b.mi->B->d_S, 1, d_res, d_cig + 2, cap, d_used);
-			unsigned long long used = 0;
+			mmb_ksw_enqueue(ctx, K);
+			// (pinned: a copy to pageable memory would wait for the stream in a spin loop)
+			unsigned long long *h_used = bb.h_used.as<unsigned long long>(1);
 			MMB_CUDA_CHECK(cudaMemcpyAsync(&res[c0], d_res, sizeof(mmb_ksw_res_t) * m, cudaMemcpyDeviceToHost, ctx->stream));
-			MMB_CUDA_CHECK(cudaMemcpyAsync(&used, d_used, 8, cudaMemcpyDeviceToHost, ctx->stream));
-			MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-			if ((int64_t)used > cap) { cap = (int64_t)used + 16; continue; } // rare: rerun the chunk with a larger CIGAR arena
+			MMB_CUDA_CHECK(cudaMemcpyAsync(h_used, d_used, 8, cudaMemcpyDeviceToHost, ctx->stream));
+			mmb_tl(ctx, MMB_TL_ENQUEUED, 1);
+			mmb_stream_sync(ctx);
+			const unsigned long long used = *h_used;
+			if ((int64_t)used > cap) { cap = (int64_t)used + 16; gatew.drop(); continue; } // rare: rerun the chunk with a larger CIGAR arena
 			if (cig_fill + (int64_t)used > cap_tot) { // grow the wave's host staging buffer, keeping the chunks already staged
 				int64_t rest = 0;
 				for (int64_t i = c0 + m; i < n_jobs; ++i) rest += cig_est(jobs[i]);
@@ -831,13 +852,13 @@ static int64_t ksw_wave(Batch &b, const std::vector<int> &active, const mmb_ksw_
 			++b.keep_used;
 			if (used) MMB_CUDA_CHECK(cudaMemcpyAsync(h_cig + cig_fill, d_cig + 2, used * 4, cudaMemcpyDeviceToHost, ctx->stream));
 			cig_fill += (int64_t)used;
-			MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+			mmb_stream_sync(ctx);
+			gatew.drop();
 			break;
 		}
 	}
-	gatew.drop();
-	b.lap("  wave gpu");
 	// hand the results to the per-read caches (pointers only)
+	HostSpan hs_(ctx, HPH_SCATTER);
 	parallel_for((int64_t)active.size(), b.n_threads, [&](int64_t t, int) {
 		ReadState &r = rs[active[t]];
 		if (r.done) return;
@@ -868,6 +889,7 @@ static void align_waves(Batch &b)
 	fpar.q = (int8_t)b.opt->q, fpar.e = (int8_t)b.opt->e, fpar.log_gap = 1;
 	while (!active.empty()) {
 		// replay every active read; collect the jobs they miss
+		mmb_tl(b.ctx, MMB_TL_HOST_BEGIN, HPH_REPLAY);
 		parallel_for((int64_t)active.size(), b.n_threads, [&](int64_t t, int) {
 			hl_hp_flush();
 			ReadState &r = rs[active[t]];
@@ -883,10 +905,9 @@ static void align_waves(Batch &b)
 			else if (ra.defer && !ra.fin_hits.empty()) r.n_regs = n_regs, r.regs = regs, r.fin_pending = true;
 			else post_align(b, r, n_regs, regs);
 		});
-		b.lap("  wave replay");
+		mmb_tl(b.ctx, MMB_TL_HOST_END, HPH_REPLAY);
 		device_tail(b, active, fpar);
 		const int64_t n_jobs = ksw_wave(b, active, sc);
-		b.lap("  wave scatter");
 		std::vector<int> still;
 		for (size_t t = 0; t < active.size(); ++t) if (!rs[active[t]].done) still.push_back(active[t]);
 		if (!still.empty() && n_jobs == 0) { fprintf(stderr, "[ERROR] minimap2_b200: alignment scheduler made no progress\n"); abort(); }
@@ -901,6 +922,7 @@ static void finalize_batch(Batch &b, int *n_regs_out, mm_reg1_t **regs_out, int 
 	std::vector<ReadState> &rs = b.bb.rs_pool;
 	const std::vector<int> &live = b.live;
 	const mm_mapopt_t *opt = b.opt;
+	HostSpan hs_(b.ctx, HPH_FINALIZE);
 	parallel_for(b.n, b.n_threads, [&](int64_t j, int) {
 		hl_hp_flush();
 		ReadState &r = rs[live[j]];
@@ -928,22 +950,16 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 	for (int t = 0; t < 2; ++t) // splice scores (mm_idx_spsc_read): what mm_idx_spsc_get feeds ksw_exts2 (align.c:640)
 		ctx->n_spsc[t] = B->n_spsc[t], ctx->spsc_pos[t] = (const int64_t*)B->d_spsc[t], ctx->spsc_val[t] = B->d_spsc[t]? B->d_spsc[t] + B->n_spsc[t] * 8 : nullptr;
 	if (!take_reads(b, n_reads, qlens, seqs, names, n_regs_out, regs_out, rep_len_out)) return 0;
-	b.lap("setup");
 	const uint8_t *h_seq = upload_reads(G, b);
 	// the reads are on their way before the group queues for a device slot: every group's upload starts when the batch starts and
 	// overlaps the kernels of the groups ahead of it
-	GateHold gate1(b.gated, 0);
-	b.lap("gate wait 1");
+	GateHold gate1(ctx, b.gated, 0);
 	seed_batch(b, h_seq, names, pass.occ_cut);
-	b.lap("h2d+sketch+seed+sort");
 	chain_batch(b, pass, gate1);
-	b.lap("chain+rescue+d2h");
 	chains_to_hits(b, pass);
 	if (opt->flag & MM_F_CIGAR) align_waves(b);
-	b.lap("waves end");
 	finalize_batch(b, n_regs_out, regs_out, rep_len_out);
-	b.lap("finalize");
-	if (Lap::on()) hl_hp_dump("group");
+	if (g_hp_on) hl_hp_dump("group");
 	return 0;
 }
 
@@ -1005,8 +1021,20 @@ mmb_ctx_t *mmb_default_ctx(void);
 void mmb_register_ctx(mmb_ctx_t *c);
 
 static int g_groups_override = 0;
-extern "C" void mmb_set_gpu_slots(int n) { g_gpu_slots = n < 1? 1 : n; }
+extern "C" void mmb_set_gpu_slots(int n) { g_gpu_slots = n < 1? g_gpu_slots_env : n; } // 0 = default (MM_B200_GPU_SLOTS or two thirds of the groups)
 extern "C" void mmb_set_groups(int n) { g_groups_override = n; } // 0 = default (MM_B200_GROUPS or 12); negative: that many groups, one after another
+
+// The scheduler timeline of scheduler group `group` for the last mm_map_batch call (mmb_timeline_enable(1) first): copies up to cap
+// (time, event, argument) triples to out (3 doubles each) and returns how many there are; -1 for a group that does not exist.
+extern "C" int64_t mmb_timeline_get(int group, double *out, int64_t cap)
+{
+	std::lock_guard<std::mutex> lk(g_group_mu);
+	if (group < 0 || group >= MAX_GROUPS || !g_groups[group]) return -1;
+	const std::vector<double> &tl = g_groups[group]->ctx->tl;
+	const int64_t n = (int64_t)tl.size() / 3;
+	if (out) std::copy(tl.begin(), tl.begin() + 3 * std::min(n, std::max<int64_t>(cap, 0)), out);
+	return n;
+}
 
 static GroupCtx &get_group(int g, int device)
 {
@@ -1036,7 +1064,8 @@ static int map_batch_pass(const mm_idx_t *mi, int n_reads, const int *qlens, con
 	for (int i = 0; i < n_reads; ++i) total += qlens[i] > 0? qlens[i] : 0;
 	if (n_reads < 64 * NG || total < 4000000) NG = 1;
 	const int device = mi->B->ctx->device;
-	for (int g = 0; g < NG; ++g) { GroupCtx &gc = get_group(g, device); gc.ctx->profiling = mmb_default_ctx()->profiling; gc.gated = NG > 1 && !sequential; }
+	for (int g = 0; g < NG; ++g) { GroupCtx &gc = get_group(g, device); gc.ctx->profiling = mmb_default_ctx()->profiling; gc.gated = gc.ctx->sleepy_sync = NG > 1 && !sequential; }
+	g_batch_groups = NG;
 	if (NG == 1) return map_group(get_group(0, device), mi, n_reads, qlens, seqs, names, n_regs_out, regs_out, rep_len_out, opt, n_threads, pass);
 	std::vector<int> cut(NG + 1, 0);
 	{
@@ -1075,7 +1104,21 @@ extern "C" int mm_map_batch(const mm_idx_t *mi, int n_reads, const int *qlens, c
 	if (n_reads <= 0) return 0;
 	static std::mutex batch_mu; // the scheduler groups (streams, arenas) are process-wide: concurrent callers take turns
 	std::lock_guard<std::mutex> batch_lk(batch_mu);
-	g_batch_t0 = realtime();
+	static std::once_flag heap_once;
+	std::call_once(heap_once, []() {
+		// Keep freed heap memory in the process. Every batch allocates and frees the same few GB on the host threads (hits,
+		// CIGARs, job lists of up to a few MB); with glibc's defaults the large blocks are mmap'd and unmapped each time and the heap
+		// top is trimmed, so the next batch takes its page faults again, serialised on the process's address-space lock, and
+		// the host phases of all groups slow down together (map-ont on an H100 host with 16 CPUs: steps whose host phases took
+		// 2-4 times as long as usual, 60-190 ms with the device idle; none with these settings).
+		mallopt(M_MMAP_THRESHOLD, 32 << 20);
+		mallopt(M_TRIM_THRESHOLD, INT_MAX);
+		mallopt(M_TOP_PAD, 256 << 20);
+	});
+	if (g_mmb_tl_on) { // the timeline holds the current batch only
+		std::lock_guard<std::mutex> lk(g_group_mu);
+		for (GroupCtx *g : g_groups) if (g) g->ctx->tl.clear();
+	}
 	if (!supported_mode(mi, opt)) { // mm_map / mm_map_frag report no hits, mm_map_file returns the error (main.c:389 exits on it)
 		for (int i = 0; i < n_reads; ++i) { n_regs_out[i] = 0, regs_out[i] = nullptr; if (rep_len_out) rep_len_out[i] = 0; }
 		return -1;

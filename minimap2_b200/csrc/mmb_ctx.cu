@@ -1,6 +1,7 @@
 // minimap2_b200/csrc/mmb_ctx.cu -- device context + kernel-level C-ABI entry points with host buffers (mm_b200.h).
 #include "mmb_internal.h"
 #include <cstring>
+#include <ctime>
 
 int mm_verbose_dummy_anchor = 0;
 
@@ -14,6 +15,16 @@ extern "C" int mmb_device_count(void)
 	}
 	return n;
 }
+
+bool g_mmb_tl_on = false;
+double mmb_tl_now()
+{
+	timespec ts;
+	clock_gettime(CLOCK_MONOTONIC, &ts);
+	return (double)ts.tv_sec + 1e-9 * (double)ts.tv_nsec;
+}
+extern "C" void mmb_timeline_enable(int on) { g_mmb_tl_on = on != 0; }
+extern "C" double mmb_timeline_now(void) { return mmb_tl_now(); }
 
 #include <mutex>
 static std::vector<mmb_ctx_t*> g_all_ctx;
@@ -37,6 +48,7 @@ extern "C" mmb_ctx_t *mmb_ctx_create(int device)
 	MMB_CUDA_CHECK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
 	MMB_CUDA_CHECK(cudaEventCreate(&c->ev0));
 	MMB_CUDA_CHECK(cudaEventCreate(&c->ev1));
+	MMB_CUDA_CHECK(cudaEventCreate(&c->ev_sync));
 	return c;
 }
 
@@ -47,7 +59,7 @@ extern "C" void mmb_ctx_destroy(mmb_ctx_t *c)
 	cudaStreamSynchronize(c->stream);
 	c->d_a.release(); c->d_b.release(); c->d_c.release(); c->d_d.release();
 	c->d_e.release(); c->d_f.release(); c->d_g.release(); c->d_h.release(); c->sk_pk.release(); c->sk_nm.release(); c->sk_misc.release(); c->scan_sums.release(); c->d_junc.release(); c->d_spsc[0].release(); c->d_spsc[1].release();
-	cudaEventDestroy(c->ev0); cudaEventDestroy(c->ev1);
+	cudaEventDestroy(c->ev0); cudaEventDestroy(c->ev1); cudaEventDestroy(c->ev_sync);
 	cudaStreamDestroy(c->stream);
 	delete c;
 }

@@ -6,6 +6,8 @@
 #include <cstdlib>
 #include <vector>
 #include <utility>
+#include <chrono>
+#include <thread>
 #include "mm_b200.h"
 
 extern "C" int mm_verbose;
@@ -79,7 +81,43 @@ struct mmb_ctx_s {
 	// entry per position: the largest byte) in target coordinates and their bytes (score+64)<<1 | acceptor
 	const int64_t *spsc_pos[2] = {nullptr, nullptr}; const uint8_t *spsc_val[2] = {nullptr, nullptr}; int64_t n_spsc[2] = {0, 0};
 	DevBuf d_spsc[2];
+	std::vector<double> tl;                   // scheduler timeline of the current batch: (time, event, argument) triples, see mmb_tl
+	cudaEvent_t ev_sync = nullptr;            // the event mmb_stream_sync polls
+	bool sleepy_sync = false;                 // mmb_stream_sync sleeps between polls (a scheduler group running next to others)
 };
+
+// Scheduler timeline (mmb_timeline_enable): the host clock (CLOCK_MONOTONIC, seconds) at each phase boundary of a group's batch.
+// Recording takes no lock and never synchronises, so the schedule it observes is the one that runs without it.
+enum {
+	MMB_TL_GATE_REQ = 0,   // argument: gate class (0 stage 1, 1 alignment wave)
+	MMB_TL_GATE_GRANT = 1, // argument: gate class
+	MMB_TL_GATE_REL = 2,   // argument: gate class
+	MMB_TL_ENQUEUED = 3,   // the device work of a phase is on the stream; argument: 0 stage 1, 1 wave chunk, 2 device tail
+	MMB_TL_SYNC = 4,       // a stream synchronise returned
+	MMB_TL_HOST_BEGIN = 5, // argument: host phase (map.cu, HostPhase)
+	MMB_TL_HOST_END = 6,
+};
+extern bool g_mmb_tl_on;
+double mmb_tl_now();
+inline void mmb_tl(mmb_ctx_t *c, int ev, int arg = 0)
+{
+	if (g_mmb_tl_on) c->tl.push_back(mmb_tl_now()), c->tl.push_back(ev), c->tl.push_back(arg);
+}
+// Waits until the work on the context's stream is done, recorded on the timeline. A scheduler group that runs next to others
+// (sleepy_sync) sleeps between polls instead of spinning as cudaStreamSynchronize does: the groups that hold a device slot wait here
+// most of the time, and spinning threads would take the host CPUs the other groups' host phases run on. A wait then ends up to
+// about 1 ms late (measured on an H100 host), which the concurrent groups cover; a context running alone spins, so that the
+// per-kernel CUDA-event times of a serialised run do not take in the late wake-ups.
+inline void mmb_stream_sync(mmb_ctx_t *c)
+{
+	if (c->sleepy_sync) {
+		MMB_CUDA_CHECK(cudaEventRecord(c->ev_sync, c->stream));
+		cudaError_t st;
+		while ((st = cudaEventQuery(c->ev_sync)) == cudaErrorNotReady) std::this_thread::sleep_for(std::chrono::microseconds(20));
+		MMB_CUDA_CHECK(st);
+	} else MMB_CUDA_CHECK(cudaStreamSynchronize(c->stream));
+	mmb_tl(c, MMB_TL_SYNC);
+}
 
 // Timing of one kernel family on the ctx stream with CUDA events (only when profiling is enabled). Asynchronous: the event
 // pairs are queued and resolved by mmb_profile_ms(), so enabling profiling does not serialise the pipeline.

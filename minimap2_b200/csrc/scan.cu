@@ -93,6 +93,6 @@ int64_t mmb_exclusive_scan_i64(mmb_ctx_t *ctx, int64_t *d, int64_t n, bool with_
 	mmb_exclusive_scan_i64_async(ctx, d, n);
 	int64_t total = 0;
 	MMB_CUDA_CHECK(cudaMemcpyAsync(&total, d + (n > 0? n : 0), sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-	MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+	mmb_stream_sync(ctx);
 	return total;
 }

@@ -548,7 +548,7 @@ int64_t mmb_sketch_device(mmb_ctx_t *ctx, const uint8_t *d_bytes, const uint32_t
 			MMB_CUDA_CHECK(cudaGetLastError());
 			++ctx->n_launch;
 			MMB_CUDA_CHECK(cudaMemcpyAsync(&total, A.tile_excl + n_tiles, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-			MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+			mmb_stream_sync(ctx);
 			if (total <= cap) break;
 			cap = total + 16;
 		}
