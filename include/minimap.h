@@ -99,7 +99,7 @@ typedef struct {
 } mm_idx_seq_t;
 
 /* the index (minimap.h:88-100). B is opaque: here it points at the device index object (host lookup arrays + the
- * HBM-resident mirror); I/spsc/J are unused by this implementation and stay NULL. */
+ * HBM-resident mirror); I, spsc and J are the annotation tables of mm_idx_bed_read, mm_idx_spsc_read2 and mm_idx_jjump_read. */
 typedef struct {
 	int32_t b, w, k, flag;
 	uint32_t n_seq;
@@ -256,7 +256,7 @@ int mm_idx_getseq(const mm_idx_t *mi, uint32_t rid, uint32_t st, uint32_t en, ui
 const uint64_t *mm_idx_get(const mm_idx_t *mi, uint64_t minier, int *n);              /* mmpriv.h:96, index.c:93 */
 int32_t mm_idx_cal_max_occ(const mm_idx_t *mi, float f);                              /* mmpriv.h:97, index.c:198 */
 
-/* optional index annotations (index.c:642-1074): not on the hot path; accepted and ignored with a warning */
+/* optional index annotations (index.c:642-1074) */
 int mm_idx_alt_read(mm_idx_t *mi, const char *fn);                                    /* minimap.h:413 */
 int mm_idx_bed_read(mm_idx_t *mi, const char *fn, int read_junc);                     /* minimap.h:414 */
 int mm_idx_bed_junc(const mm_idx_t *mi, int32_t ctg, int32_t st, int32_t en, uint8_t *s); /* minimap.h:415 */
@@ -264,6 +264,11 @@ int mm_max_spsc_bonus(const mm_mapopt_t *mo);                                   
 int32_t mm_idx_spsc_read(mm_idx_t *idx, const char *fn, int32_t max_sc);              /* minimap.h:418 */
 int32_t mm_idx_spsc_read2(mm_idx_t *idx, const char *fn, int32_t max_sc, float scale);/* minimap.h:419 */
 int64_t mm_idx_spsc_get(const mm_idx_t *db, int32_t cid, int64_t st0, int64_t en0, int32_t rev, uint8_t *sc); /* minimap.h:420 */
+/* junctions that spliced hits may jump across (index.c:903-930): flag MM_JUNC_ANNO for annotation, MM_JUNC_MISC for junctions of a
+ * first pass (--write-junc output, lines scoring at least min_sc). A second call merges into the table. -1: the file cannot be read. */
+#define MM_JUNC_ANNO 0x1 /* mmpriv.h:27-28 */
+#define MM_JUNC_MISC 0x2
+int mm_idx_jjump_read(mm_idx_t *mi, const char *fn, int flag, int min_sc);             /* mmpriv.h:95 */
 
 /* thread buffers (map.c:13-31) */
 mm_tbuf_t *mm_tbuf_init(void);                                                        /* minimap.h:351 */

@@ -165,6 +165,28 @@ int mmb_tail_batch_host(mmb_ctx_t *ctx, int n_hits, const mmb_tail_hit_t *hits, 
 						const int64_t *cig_off, mmb_tail_out_t *out, uint32_t *cigar_out);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * K5: junction jumps of spliced hits on the device   (the decisions of mm_jump_split, jump.c:50-201)
+ * --------------------------------------------------------------------------------------------------------- */
+typedef struct {
+	int32_t rid, rs, re, qs, qe, rev; /* the hit (mm_reg1_t fields) */
+	int32_t qlen, n_cigar;            /* read length; the hit's CIGAR length */
+	int64_t q_off;                    /* offset of the read's first base in the batch's bases */
+	uint32_t cig_first, cig_last;     /* first and last CIGAR words */
+} mmb_jump_hit_t;
+typedef struct {
+	int32_t act;          /* 0: nothing, 1: trim the end back to the splice site, 2: add an exon across the junction */
+	int32_t l, off, off2; /* l as jump.c computes it; the chosen jump-table entry */
+	int32_t mm0;          /* mismatches of the chosen candidate */
+} mmb_jump_side_t;
+typedef struct { mmb_jump_side_t side[2]; } mmb_jump_dec_t; /* [0]: left end of the alignment, [1]: right end (decided after [0]) */
+/* Kernel-level entry: K5 on n_hits hits against the jump table of mi (mm_idx_jjump_read), reads given as ASCII back to back
+ * (off[n_reads+1]); opt supplies a, b and jump_min_match. Returns 0, or -1 when mi has no jump table. */
+int mmb_jump_batch_host(mmb_ctx_t *ctx, const mm_idx_t *mi, const mm_mapopt_t *opt, int n_reads, const char *seqs, const int64_t *off,
+						int n_hits, const mmb_jump_hit_t *hits, mmb_jump_dec_t *out);
+/* The host half of mm_jump_split: applies one hit's decisions (left, then right) to r and its libc-owned r->p. */
+void mmb_jump_apply(const mm_mapopt_t *opt, int qlen, mm_reg1_t *r, const mmb_jump_dec_t *d);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Index on device + whole-path batch mapping are driven through the minimap.h API (include/minimap.h):
  * mm_idx_* builds/loads the index on the GPU (side table keyed by mm_idx_t*), mm_map_file / mm_map_batch run the GPU
  * batch scheduler that replaces worker_pipeline/kt_for (map.c:403-691). The entries below are the knobs and hand-off

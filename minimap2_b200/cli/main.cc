@@ -43,7 +43,7 @@ static struct option long_options[] = {
 	{ "score-N", required_argument, 0, 331 }, { "eqx", no_argument, 0, 332 }, { "paf-no-hit", no_argument, 0, 333 },
 	{ "no-end-flt", no_argument, 0, 335 }, { "hard-mask-level", no_argument, 0, 336 }, { "cap-sw-mem", required_argument, 0, 337 },
 	{ "max-qlen", required_argument, 0, 338 }, { "max-chain-iter", required_argument, 0, 339 }, { "sam-hit-only", no_argument, 0, 342 },
-	{ "chain-gap-scale", required_argument, 0, 343 }, { "junc-bed", required_argument, 0, 340 }, { "junc-bonus", required_argument, 0, 341 }, { "junc-pen", required_argument, 0, 358 }, { "spsc", required_argument, 0, 357 }, { "spsc-scale", required_argument, 0, 363 }, { "spsc0", required_argument, 0, 364 }, { "alt", required_argument, 0, 344 }, { "alt-drop", required_argument, 0, 345 }, { "mask-len", required_argument, 0, 346 },
+	{ "chain-gap-scale", required_argument, 0, 343 }, { "junc-bed", required_argument, 0, 340 }, { "junc-bonus", required_argument, 0, 341 }, { "junc-pen", required_argument, 0, 358 }, { "spsc", required_argument, 0, 357 }, { "jump-min-match", required_argument, 0, 360 }, { "write-junc", no_argument, 0, 361 }, { "pass1", required_argument, 0, 362 }, { "spsc-scale", required_argument, 0, 363 }, { "spsc0", required_argument, 0, 364 }, { "alt", required_argument, 0, 344 }, { "alt-drop", required_argument, 0, 345 }, { "mask-len", required_argument, 0, 346 },
 	{ "rmq", optional_argument, 0, 347 }, { "q-occ-frac", required_argument, 0, 350 }, { "chain-skip-scale", required_argument, 0, 351 },
 	{ "no-hash-name", no_argument, 0, 353 }, { "secondary-seq", no_argument, 0, 354 }, { "ds", no_argument, 0, 355 },
 	{ "rmq-inner", required_argument, 0, 356 }, { "help", no_argument, 0, 'h' }, { "version", no_argument, 0, 'V' },
@@ -59,7 +59,7 @@ int main(int argc, char *argv[])
 	mm_mapopt_t opt;
 	mm_idxopt_t ipt;
 	int c, n_threads = 3, old_best_n = -1, li = 0;
-	char *fnw = 0, *s, *alt_list = 0, *fn_bed_junc = 0, *fn_spsc = 0, *rg = 0;
+	char *fnw = 0, *s, *alt_list = 0, *fn_bed_junc = 0, *fn_bed_jump = 0, *fn_bed_pass1 = 0, *fn_spsc = 0, *rg = 0;
 	float spsc_scale = 0.7f;
 	mm_verbose = 3;
 	mm_realtime0 = realtime();
@@ -114,10 +114,7 @@ int main(int argc, char *argv[])
 			else if (t == 1) opt.flag &= ~MM_F_SPLICE_OLD;
 		}
 		else if (c == 'R') rg = optarg; // SAM read group line (main.c:199; written by mm_write_sam_hdr, repeated as RG:Z: on every record)
-		else if (c == 'j') { // accepted by the reference, not built here: refuse instead of silently ignoring
-			fprintf(stderr, "[ERROR] option -j (junction jump BED for short RNA-seq reads) is not supported by minimap2-b200\n");
-			return 1;
-		}
+		else if (c == 'j') fn_bed_jump = optarg; // annotated junctions to jump across (main.c:202)
 		else if (c == 'I') ipt.batch_size = parse_num(optarg);
 		else if (c == 'K') opt.mini_batch_size = parse_num(optarg);
 		else if (c == 'e') opt.occ_dist = (int)parse_num(optarg);
@@ -162,6 +159,9 @@ int main(int argc, char *argv[])
 		else if (c == 358 || c == 364) opt.junc_pen = atoi(optarg);
 		else if (c == 357) fn_spsc = optarg;
 		else if (c == 363) spsc_scale = (float)atof(optarg);
+		else if (c == 360) opt.jump_min_match = (int)parse_num(optarg); // main.c:261-263
+		else if (c == 361) opt.flag |= MM_F_OUT_JUNC | MM_F_CIGAR;
+		else if (c == 362) fn_bed_pass1 = optarg;
 		else if (c == 344) alt_list = optarg;
 		else if (c == 345) opt.alt_drop = atof(optarg);
 		else if (c == 346) opt.mask_len = (int)parse_num(optarg);
@@ -233,6 +233,14 @@ int main(int argc, char *argv[])
 		if (fn_bed_junc) { // main.c:467-471
 			mm_idx_bed_read(mi, fn_bed_junc, 1);
 			if (mi->I == 0 && mm_verbose >= 2) fprintf(stderr, "[WARNING] failed to load the junction BED file\n");
+		}
+		if (fn_bed_jump) { // main.c:472-481: annotated junctions, then pass-1 junctions scoring at least 5, merged into one table
+			mm_idx_jjump_read(mi, fn_bed_jump, MM_JUNC_ANNO, -1);
+			if (mi->J == 0 && mm_verbose >= 2) fprintf(stderr, "[WARNING] failed to load the jump BED file\n");
+		}
+		if (fn_bed_pass1) {
+			mm_idx_jjump_read(mi, fn_bed_pass1, MM_JUNC_MISC, 5);
+			if (mi->J == 0 && mm_verbose >= 2) fprintf(stderr, "[WARNING] failed to load the pass-1 jump BED file\n");
 		}
 		if (fn_spsc) { // main.c:482-486
 			mm_idx_spsc_read2(mi, fn_spsc, mm_max_spsc_bonus(&opt), spsc_scale);

@@ -143,6 +143,111 @@ static inline int mmx_bed_junc(const mm_idx_intv_s *I, int32_t n_seq, int32_t ct
 	return left;
 }
 
+// ---- junction jumps (mm_idx_t::J; index.c:828-959) ----
+#ifndef MM_JUNC_ANNO
+#define MM_JUNC_ANNO 0x1 // mmpriv.h:27-28
+#define MM_JUNC_MISC 0x2
+#endif
+typedef struct { // mmpriv.h:59-63; also the entry of the device table (index.h: d_jump)
+	int32_t off, off2, cnt;
+	int16_t strand;
+	uint16_t flag;
+} mm_idx_jjump1_t;
+struct mm_idx_jjump_s { // one per contig: both ends of every intron, sorted by (off, off2), equal pairs merged
+	int32_t n, m;
+	mm_idx_jjump1_t *a;
+};
+struct MmxKeyJjOff  { MM_HD uint64_t operator()(const mm_idx_jjump1_t &v) const { return (uint64_t)(uint32_t)v.off; } };  // sort_key_jj, index.c:832
+struct MmxKeyJjOff2 { MM_HD uint64_t operator()(const mm_idx_jjump1_t &v) const { return (uint64_t)(uint32_t)v.off2; } }; // sort_key_jj2, index.c:835
+
+// sort_jjump (index.c:838-863). Both radix sorts have 4-byte keys; mmx_rs_sort starts at the most significant byte in which the
+// keys differ, which for keys below 2^32 is the walk a 4-byte sort takes. The merged entry keeps the strand of the first entry of
+// its run, so the unstable order of equal keys is replayed, not just the sorted result.
+static inline void mmx_jjump_sort(mm_idx_jjump_s *jj)
+{
+	if (jj->n == 0) return;
+	std::vector<int32_t> stk((size_t)mmx_rs_stack_len(jj->n));
+	mmx_rs_sort(jj->a, (int64_t)jj->n, stk.data(), MmxKeyJjOff());
+	for (int32_t j0 = 0, j = 1; j <= jj->n; ++j)
+		if (j == jj->n || jj->a[j0].off != jj->a[j].off) {
+			mmx_rs_sort(jj->a + j0, (int64_t)(j - j0), stk.data(), MmxKeyJjOff2());
+			j0 = j;
+		}
+	int32_t k = 0;
+	for (int32_t j0 = 0, j = 1; j <= jj->n; ++j)
+		if (j == jj->n || jj->a[j0].off != jj->a[j].off || jj->a[j0].off2 != jj->a[j].off2) {
+			int32_t cnt = 0;
+			uint16_t flag = 0;
+			for (int32_t t = j0; t < j; ++t) cnt += jj->a[t].cnt, flag |= jj->a[t].flag;
+			jj->a[k] = jj->a[j0];
+			jj->a[k].cnt = cnt;
+			jj->a[k++].flag = flag;
+			j0 = j;
+		}
+	jj->n = jj->m = k;
+}
+
+// mm_idx_bed2jjump (index.c:865-883): each intron as {off=st, off2=en} and {off=en, off2=st}
+static inline mm_idx_jjump_s *mmx_bed2jjump(const mm_idx_intv_s *I, uint32_t n_seq, uint16_t flag)
+{
+	mm_idx_jjump_s *J = (mm_idx_jjump_s*)calloc(n_seq, sizeof(mm_idx_jjump_s));
+	for (uint32_t i = 0; i < n_seq; ++i) {
+		const mm_idx_intv_s *v = &I[i];
+		mm_idx_jjump_s *jj = &J[i];
+		jj->n = jj->m = v->n * 2;
+		jj->a = (mm_idx_jjump1_t*)calloc(jj->n > 0? jj->n : 1, sizeof(mm_idx_jjump1_t));
+		for (int32_t j = 0, k = 0; j < v->n; ++j) {
+			const mm_idx_intv1_t &t = v->a[j];
+			jj->a[k].off = t.st, jj->a[k].off2 = t.en, jj->a[k].cnt = t.cnt, jj->a[k].strand = (int16_t)t.strand, jj->a[k++].flag = flag;
+			jj->a[k].off = t.en, jj->a[k].off2 = t.st, jj->a[k].cnt = t.cnt, jj->a[k].strand = (int16_t)t.strand, jj->a[k++].flag = flag;
+		}
+		mmx_jjump_sort(jj);
+	}
+	return J;
+}
+
+// mm_idx_jjump_merge (index.c:885-901): J0's entries, then J1's, through the same sort; J0 and J1 are freed
+static inline mm_idx_jjump_s *mmx_jjump_merge(mm_idx_jjump_s *J0, mm_idx_jjump_s *J1, uint32_t n_seq)
+{
+	mm_idx_jjump_s *J2 = (mm_idx_jjump_s*)calloc(n_seq, sizeof(mm_idx_jjump_s));
+	for (uint32_t i = 0; i < n_seq; ++i) {
+		mm_idx_jjump_s *jj = &J2[i];
+		jj->n = jj->m = J0[i].n + J1[i].n;
+		jj->a = (mm_idx_jjump1_t*)calloc(jj->n > 0? jj->n : 1, sizeof(mm_idx_jjump1_t));
+		if (J0[i].n) memcpy(jj->a, J0[i].a, sizeof(mm_idx_jjump1_t) * J0[i].n);
+		if (J1[i].n) memcpy(jj->a + J0[i].n, J1[i].a, sizeof(mm_idx_jjump1_t) * J1[i].n);
+		mmx_jjump_sort(jj);
+		free(J0[i].a), free(J1[i].a);
+	}
+	free(J0), free(J1);
+	return J2;
+}
+
+// mm_idx_jump_get_core (index.c:932-944): the last entry with off <= x, -1 if there is none
+MM_HD int32_t mmx_jump_get_core(int32_t n, const mm_idx_jjump1_t *a, int32_t x)
+{
+	int32_t s = 0, e = n;
+	if (n == 0 || x < a[0].off) return -1;
+	while (s < e) {
+		const int32_t mid = s + (e - s) / 2;
+		if (x >= a[mid].off && (mid + 1 >= n || x < a[mid + 1].off)) return mid;
+		else if (x < a[mid].off) e = mid;
+		else s = mid + 1;
+	}
+	return n - 1; // not reached: a is sorted by off
+}
+
+// mm_idx_jump_get (index.c:946-959): the entries of one contig with off in (st, en], en clamped to the contig length
+MM_HD const mm_idx_jjump1_t *mmx_jump_get(int32_t n_a, const mm_idx_jjump1_t *a, int32_t seq_len, int32_t st, int32_t en, int32_t *n)
+{
+	*n = 0;
+	if (en < 0 || en > seq_len) en = seq_len;
+	if (n_a == 0) return 0;
+	const int32_t l = mmx_jump_get_core(n_a, a, st), r = mmx_jump_get_core(n_a, a, en);
+	*n = r - l;
+	return &a[l + 1];
+}
+
 // ---- splice scores (mm_idx_t::spsc; index.c:963-1075) ----
 struct mm_idx_spsc_s { // index.c:963-966; one entry per (contig, strand): a[] = pos<<8 | (score+64)<<1 | acceptor, sorted
 	uint32_t n, m;

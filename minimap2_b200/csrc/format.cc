@@ -169,6 +169,41 @@ extern "C" int mm_gen_cs(void *, char **buf, int *max_len, const mm_idx_t *mi, c
 extern "C" int mm_gen_ds(void *, char **buf, int *max_len, const mm_idx_t *mi, const mm_reg1_t *r, const char *seq, int no_iden) { return gen_tag(buf, max_len, mi, r, seq, 0, 1, no_iden); }
 extern "C" int mm_gen_MD(void *, char **buf, int *max_len, const mm_idx_t *mi, const mm_reg1_t *r, const char *seq) { return gen_tag(buf, max_len, mi, r, seq, 1, 0, 0); }
 
+// mm_write_junc (format.c:256-300): one BED6 line per intron of a spliced hit with a preferred transcript strand (contig, start, end,
+// read name, donor + acceptor score, strand), each ended by a newline
+void hl_write_junc(std::string &s, const mm_idx_t *mi, const char *qname, const mm_reg1_t *r)
+{
+	if (!r->is_spliced || r->p == 0) return;
+	if (r->p->trans_strand != 1 && r->p->trans_strand != 2) return;
+	auto revcomp_splice = [](uint8_t x[2]) { const uint8_t c = x[1] < 4? 3 - x[1] : 4; x[1] = x[0] < 4? 3 - x[0] : 4; x[0] = c; };
+	int32_t t_off = r->rs;
+	for (uint32_t i = 0; i < r->p->n_cigar; ++i) {
+		const int op = r->p->cigar[i] & 0xf, len = (int)(r->p->cigar[i] >> 4);
+		if (op == MM_CIGAR_MATCH || op == MM_CIGAR_EQ_MATCH || op == MM_CIGAR_X_MISMATCH || op == MM_CIGAR_DEL) t_off += len;
+		else if (op == MM_CIGAR_N_SKIP) {
+			uint8_t donor[2], acceptor[2];
+			int score1 = 0, score2 = 0;
+			const int rev = (r->p->trans_strand == 2) ^ r->rev;
+			if (!rev) {
+				mm_idx_getseq(mi, r->rid, t_off, t_off + 2, donor);
+				mm_idx_getseq(mi, r->rid, t_off + len - 2, t_off + len, acceptor);
+			} else {
+				mm_idx_getseq(mi, r->rid, t_off, t_off + 2, acceptor);
+				mm_idx_getseq(mi, r->rid, t_off + len - 2, t_off + len, donor);
+				revcomp_splice(donor), revcomp_splice(acceptor);
+			}
+			if (donor[0] == 2 && donor[1] == 3) score1 = 3;
+			else if (donor[0] == 2 && donor[1] == 1) score1 = 2;
+			else if (donor[0] == 0 && donor[1] == 3) score1 = 1;
+			if (acceptor[0] == 0 && acceptor[1] == 2) score2 = 3;
+			else if (acceptor[0] == 0 && acceptor[1] == 1) score2 = 1;
+			s += mi->seq[r->rid].name; s += '\t'; put_int(s, t_off); s += '\t'; put_int(s, t_off + len); s += '\t';
+			s += qname; s += '\t'; put_int(s, score1 + score2); s += '\t'; s += "+-"[rev]; s += '\n';
+			t_off += len;
+		}
+	}
+}
+
 // NB: cs/MD need the query sequence; the PAF writer receives it through hl_write_paf_seq below
 static thread_local const char *tl_seq = nullptr;
 void hl_set_seq_for_tags(const char *seq) { tl_seq = seq; }

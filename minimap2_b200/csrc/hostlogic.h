@@ -137,6 +137,7 @@ void hl_hp_dump(const char *tag);
 struct hl_str { std::string s; };
 void hl_set_seq_for_tags(const char *seq);
 void hl_write_paf(std::string &s, const mm_idx_t *mi, const char *qname, int qlen, const mm_reg1_t *r, int64_t opt_flag, int rep_len);
+void hl_write_junc(std::string &s, const mm_idx_t *mi, const char *qname, const mm_reg1_t *r);
 void hl_write_sam(std::string &s, const mm_idx_t *mi, const char *qname, const char *seq, const char *qual, int qlen, int reg_idx,
 				  int n_regs, const mm_reg1_t *regs, int64_t opt_flag, int rep_len);
 int hl_write_sam_hdr(std::string &s, const mm_idx_t *mi, const char *rg, const char *ver, int argc, char *argv[]);

@@ -283,12 +283,14 @@ extern "C" void mm_idx_destroy(mm_idx_t *mi) // index.c:62-91
 		if (B->ctx) cudaSetDevice(B->ctx->device);
 		if (!B->external) { cudaFree(B->d_tab); cudaFree(B->d_pos); cudaFree(B->d_S); cudaFree(B->d_seq_off); cudaFree(B->d_seq_len); cudaFree(B->d_cnt_sorted); } cudaFree(B->d_name_rank); cudaFree(B->d_ukeys); cudaFree(B->d_ucnt); cudaFree(B->d_uoff);
 		if (B->d_junc) cudaFree(B->d_junc);
+		if (B->d_jump_off) cudaFree(B->d_jump_off);
 		for (int t = 0; t < 2; ++t) if (B->d_spsc[t]) cudaFree(B->d_spsc[t]);
 		delete B->h_map;
 		delete B;
 	}
 	if (mi->I) { for (uint32_t i = 0; i < mi->n_seq; ++i) free(mi->I[i].a); free(mi->I); }
 	if (mi->spsc) { for (uint32_t i = 0; i < mi->n_seq * 2; ++i) free(mi->spsc[i].a); free(mi->spsc); }
+	if (mi->J) { for (uint32_t i = 0; i < mi->n_seq; ++i) free(mi->J[i].a); free(mi->J); }
 	for (uint32_t i = 0; i < mi->n_seq; ++i) free(mi->seq[i].name);
 	free(mi->seq); free(mi->S); free(mi);
 }
@@ -673,6 +675,47 @@ extern "C" int mm_idx_alt_read(mm_idx_t *mi, const char *fn) // index.c:648-670:
 	mi->n_alt = n_alt;
 	if (mm_verbose >= 3) fprintf(stderr, "[M::%s] found %d ALT contigs\n", __func__, n_alt);
 	return n_alt;
+}
+// index.c:903-930 + the device copy K5 (jump.cuh) reads. Where the reference dereferences NULL (a file that cannot be opened), this
+// returns -1 and leaves mi->J as it was.
+extern "C" int mm_idx_jjump_read(mm_idx_t *mi, const char *fn, int flag, int min_sc)
+{
+	if (mi->h == 0) mm_idx_index_name(mi);
+	mm_idx_intv_s *I = mmx_bed_read(fn, mi->n_seq, 1, min_sc, [&](const char *name) { return mm_idx_name2id(mi, name); }, nullptr, nullptr);
+	if (I == 0) return -1;
+	mm_idx_jjump_s *J = mmx_bed2jjump(I, mi->n_seq, (uint16_t)flag);
+	for (uint32_t i = 0; i < mi->n_seq; ++i) free(I[i].a);
+	free(I);
+	mi->J = mi->J? mmx_jjump_merge(mi->J, J, mi->n_seq) : J;
+	int64_t n_anno = 0, n_misc = 0;
+	std::vector<int64_t> off((size_t)mi->n_seq + 1, 0);
+	for (uint32_t i = 0; i < mi->n_seq; ++i) {
+		for (int32_t j = 0; j < mi->J[i].n; ++j)
+			if (mi->J[i].a[j].flag & MM_JUNC_ANNO) ++n_anno;
+			else ++n_misc;
+		off[i + 1] = off[i] + mi->J[i].n;
+	}
+	if (mm_verbose >= 3)
+		fprintf(stderr, "[%s] there are %d annotated and %d other splice positions in the index\n", __func__, (int)n_anno, (int)n_misc);
+	mm_idx_bucket_s *B = mi->B;
+	if (B) {
+		if (B->ctx) MMB_CUDA_CHECK(cudaSetDevice(B->ctx->device));
+		if (B->d_jump_off) { MMB_CUDA_CHECK(cudaFree(B->d_jump_off)); B->d_jump_off = nullptr, B->d_jump = nullptr; }
+		const size_t n = (size_t)off[mi->n_seq], head = ((size_t)mi->n_seq + 1) * 8;
+		MMB_CUDA_CHECK(cudaMalloc((void**)&B->d_jump_off, head + n * sizeof(mm_idx_jjump1_t) + 16));
+		B->d_jump = (mm_idx_jjump1_t*)((uint8_t*)B->d_jump_off + head);
+		MMB_CUDA_CHECK(cudaMemcpy(B->d_jump_off, off.data(), head, cudaMemcpyHostToDevice));
+		for (uint32_t i = 0; i < mi->n_seq; ++i)
+			if (mi->J[i].n) MMB_CUDA_CHECK(cudaMemcpy(B->d_jump + off[i], mi->J[i].a, sizeof(mm_idx_jjump1_t) * mi->J[i].n, cudaMemcpyHostToDevice));
+	}
+	return 0;
+}
+// index.c:946-959
+extern "C" const mm_idx_jjump1_t *mm_idx_jump_get(const mm_idx_t *mi, int32_t cid, int32_t st, int32_t en, int32_t *n)
+{
+	*n = 0;
+	if (cid >= (int32_t)mi->n_seq || cid < 0 || mi->J == 0) return 0;
+	return mmx_jump_get(mi->J[cid].n, mi->J[cid].a, (int32_t)mi->seq[cid].len, st, en, n);
 }
 // index.c:796-800 + the device copy the spliced kernel reads: introns of all contigs in global S coordinates, sorted by start
 extern "C" int mm_idx_bed_read(mm_idx_t *mi, const char *fn, int read_junc)

@@ -10,6 +10,7 @@
 #pragma once
 #include "mmb_internal.h"
 #include "minimap.h"
+#include "annot.h"
 #include <string>
 #include <unordered_map>
 #include <mutex>
@@ -46,6 +47,7 @@ struct mm_idx_bucket_s {  // the opaque "B" of mm_idx_t
 	uint64_t *d_ukeys = nullptr; uint32_t *d_ucnt = nullptr; int64_t *d_uoff = nullptr; // key list kept for the lazy host mirror
 	uint8_t *d_spsc[2] = {nullptr, nullptr}; int64_t n_spsc[2] = {0, 0}; // splice scores per strand (mm_idx_spsc_read): n positions (int64, global S coordinates) | n bytes
 	int64_t *d_junc = nullptr; int64_t n_junc = 0; // annotated introns (mm_idx_bed_read): n_junc starts | n_junc ends (global S coordinates, int64) | n_junc strands (int8)
+	int64_t *d_jump_off = nullptr; mm_idx_jjump1_t *d_jump = nullptr; // jump table (mm_idx_jjump_read): n_seq+1 entry offsets | the entries of mi->J, contig after contig (one allocation)
 	// host (lazy)
 	std::mutex mu;
 	bool host_ready = false;

@@ -7,8 +7,10 @@
 //   stage 3 (waves): host threads replay the alignment driver (align.cc) per read, the ksw2 jobs they request are run as
 //            one K3 launch set per wave, results are scattered back into per-read caches; typically 2-3 waves
 //   stage 4 (host threads): final hit selection and MAPQ
+//   stage 5 (index with a jump table only): K5 junction jumps on the device, applied to the hits on the host threads
 // Results are returned in input order with the reference's ownership rules (libc malloc, caller frees).
 #include "pipeline.h"
+#include "jump.cuh"
 #include "hostlogic.h"
 #include "scan.cuh"
 #include "ksw_plan.h"
@@ -269,6 +271,7 @@ struct BatchBufs { // device arenas reused across batches (per context)
 	PinBuf h_fin_in, h_fin_out;
 	DevBuf qlo, qhi, k_cnt;                // skip_seed inputs (ava / strand-restricted modes only)
 	DevBuf dreg, dreg_off;                 // masked intervals of the reads (-T / SDUST only)
+	DevBuf jump_io; PinBuf h_jump;         // K5 hit descriptors and decisions (jump table only)
 	PinBuf h_seq, h_misc, h_jobs, h_res, h_used;
 	std::vector<std::unique_ptr<PinBuf>> h_cig; // one CIGAR staging buffer per alignment wave (cached results point into them until the batch ends)
 	std::vector<ReadState> rs_pool;        // persistent per-read objects: their vectors keep capacity => no allocation in steady state
@@ -287,6 +290,7 @@ bool supported_mode(const mm_idx_t *mi, const mm_mapopt_t *opt)
 {
 	const char *what = nullptr;
 	if (opt->flag & (MM_F_SR | MM_F_SR_RNA)) what = "short-read mode (-x sr / splice:sr)";
+	else if (mi->J && (opt->flag & MM_F_SPLICE) && (opt->flag & MM_F_EQX)) what = "junction jumps (-j / --pass1) with =/X CIGARs (--eqx)"; // jump.c:198 asserts
 	else if ((opt->flag & MM_F_QSTRAND) && (!(opt->flag & MM_F_NO_INV) || (opt->flag & (MM_F_SPLICE | MM_F_OUT_SAM)) || (mi->flag & MM_I_HPC)))
 		what = "query-strand mode without MM_F_NO_INV (main.c:252 sets both), or combined with splice / SAM / HPC (mm_check_opt rejects those)";
 	if (what) fprintf(stderr, "[ERROR] minimap2_b200: %s is not implemented in this build; refusing to map (no CPU fallback)\n", what);
@@ -936,6 +940,70 @@ static void finalize_batch(Batch &b, int *n_regs_out, mm_reg1_t **regs_out, int 
 	});
 }
 
+// K5 launch (the kernel is in jump.cuh)
+void mmb_jump_device(mmb_ctx_t *ctx, const mm_idx_t *mi, const mm_mapopt_t *opt, int n_hits, const mmb_jump_hit_t *d_hits, const uint8_t *d_seq, mmb_jump_dec_t *d_out)
+{
+	if (n_hits <= 0) return;
+	const mm_idx_bucket_s *B = mi->B;
+	JumpArgs A;
+	A.hits = d_hits, A.n_hits = n_hits, A.seq = d_seq;
+	A.S = B->d_S, A.seq_off = B->d_seq_off, A.seq_len = B->d_seq_len;
+	A.jump_off = B->d_jump_off, A.jump = B->d_jump;
+	A.ext = 1 + (opt->b + opt->a - 1) / opt->a + 1, A.jump_min_match = opt->jump_min_match; // jump.c:55
+	A.out = d_out;
+	ProfScope ps_(ctx, MMB_PROF_OTHER, (uint64_t)n_hits);
+	jump_kernel<<<(unsigned)((n_hits + 7) / 8), 256, 0, ctx->stream>>>(A);
+	MMB_CUDA_CHECK(cudaGetLastError());
+	++ctx->n_launch;
+}
+
+// Stage 5 (map.c:362-364): junction jumps of every hit, secondaries included, after MAPQ (which they do not change). The hits whose
+// ends K5 may move go to the device as descriptors; the decisions come back and are applied here, to the hits and their CIGARs.
+static void jump_batch(Batch &b, const int *n_regs_out, mm_reg1_t *const *regs_out)
+{
+	mmb_ctx_t *ctx = b.ctx;
+	BatchBufs &bb = b.bb;
+	const std::vector<int> &live = b.live;
+	const std::vector<ReadState> &rs = bb.rs_pool;
+	std::vector<std::vector<int>> sel((size_t)b.n);
+	parallel_for(b.n, b.n_threads, [&](int64_t j, int) {
+		const int i = live[j];
+		for (int k = 0; k < n_regs_out[i]; ++k)
+			if (mmb_jump_wanted(b.mi, b.opt, rs[i].qlen, &regs_out[i][k])) sel[j].push_back(k);
+	});
+	std::vector<int64_t> hoff((size_t)b.n + 1, 0);
+	for (int j = 0; j < b.n; ++j) hoff[j + 1] = hoff[j] + (int64_t)sel[j].size();
+	const int64_t n_hits = hoff[b.n];
+	if (n_hits == 0) return;
+	const size_t in_bytes = sizeof(mmb_jump_hit_t) * (size_t)n_hits, out_bytes = sizeof(mmb_jump_dec_t) * (size_t)n_hits;
+	uint8_t *h_io = bb.h_jump.as<uint8_t>(in_bytes + out_bytes);
+	mmb_jump_hit_t *h_hits = (mmb_jump_hit_t*)h_io;
+	mmb_jump_dec_t *h_dec = (mmb_jump_dec_t*)(h_io + in_bytes);
+	parallel_for(b.n, b.n_threads, [&](int64_t j, int) {
+		const int i = live[j];
+		for (size_t t = 0; t < sel[j].size(); ++t) {
+			const mm_reg1_t *r = &regs_out[i][sel[j][t]];
+			mmb_jump_hit_t &h = h_hits[hoff[j] + (int64_t)t];
+			h.rid = r->rid, h.rs = r->rs, h.re = r->re, h.qs = r->qs, h.qe = r->qe, h.rev = r->rev;
+			h.qlen = rs[i].qlen, h.n_cigar = (int32_t)r->p->n_cigar, h.q_off = b.off[j];
+			h.cig_first = r->p->cigar[0], h.cig_last = r->p->cigar[r->p->n_cigar - 1];
+		}
+	});
+	uint8_t *d_io = bb.jump_io.as<uint8_t>(in_bytes + out_bytes);
+	{
+		GateHold gate(ctx, b.gated, 1);
+		MMB_CUDA_CHECK(cudaMemcpyAsync(d_io, h_io, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+		mmb_jump_device(ctx, b.mi, b.opt, (int)n_hits, (const mmb_jump_hit_t*)d_io, b.d_seq, (mmb_jump_dec_t*)(d_io + in_bytes));
+		MMB_CUDA_CHECK(cudaMemcpyAsync(h_dec, d_io + in_bytes, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+		mmb_stream_sync(ctx);
+	}
+	ctx->last_h2d_bytes += in_bytes, ctx->last_d2h_bytes += out_bytes;
+	parallel_for(b.n, b.n_threads, [&](int64_t j, int) {
+		const int i = live[j];
+		for (size_t t = 0; t < sel[j].size(); ++t) mmb_jump_apply(b.opt, rs[i].qlen, &regs_out[i][sel[j][t]], &h_dec[hoff[j] + (int64_t)t]);
+	});
+}
+
 static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *qlens, const char **seqs, const char **names,
 					 int *n_regs_out, mm_reg1_t **regs_out, int *rep_len_out, const mm_mapopt_t *opt, int n_threads, const MapPass &pass)
 {
@@ -959,6 +1027,7 @@ static int map_group(GroupCtx &G, const mm_idx_t *mi, int n_reads, const int *ql
 	chains_to_hits(b, pass);
 	if (opt->flag & MM_F_CIGAR) align_waves(b);
 	finalize_batch(b, n_regs_out, regs_out, rep_len_out);
+	if (mi->J && (opt->flag & MM_F_SPLICE) && (opt->flag & MM_F_CIGAR)) jump_batch(b, n_regs_out, regs_out);
 	if (g_hp_on) hl_hp_dump("group");
 	return 0;
 }
@@ -1015,6 +1084,27 @@ extern "C" int64_t mmb_seed_batch_host(mmb_ctx_t *ctx, const mm_idx_t *mi, int n
 	}
 	MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
 	return total_a;
+}
+
+extern "C" int mmb_jump_batch_host(mmb_ctx_t *ctx, const mm_idx_t *mi, const mm_mapopt_t *opt, int n_reads, const char *seqs, const int64_t *off,
+								   int n_hits, const mmb_jump_hit_t *hits, mmb_jump_dec_t *out)
+{
+	if (!mi->J || !mi->B->d_jump_off) return -1;
+	if (n_hits <= 0) return 0;
+	MMB_CUDA_CHECK(cudaSetDevice(ctx->device));
+	const int64_t total_bases = n_reads > 0? off[n_reads] : 0;
+	const size_t in_bytes = sizeof(mmb_jump_hit_t) * (size_t)n_hits, out_bytes = sizeof(mmb_jump_dec_t) * (size_t)n_hits;
+	uint8_t *d_seq = ctx->d_a.as<uint8_t>((size_t)total_bases + 16);
+	uint8_t *d_io = ctx->d_b.as<uint8_t>(in_bytes + out_bytes);
+	if (total_bases > 0) {
+		MMB_CUDA_CHECK(cudaMemcpyAsync(d_seq, seqs, total_bases, cudaMemcpyHostToDevice, ctx->stream));
+		encode_kernel<<<(unsigned)((total_bases / 4 + 256) / 256), 256, 0, ctx->stream>>>(d_seq, total_bases);
+	}
+	MMB_CUDA_CHECK(cudaMemcpyAsync(d_io, hits, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+	mmb_jump_device(ctx, mi, opt, n_hits, (const mmb_jump_hit_t*)d_io, d_seq, (mmb_jump_dec_t*)(d_io + in_bytes));
+	MMB_CUDA_CHECK(cudaMemcpyAsync(out, d_io + in_bytes, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+	MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+	return 0;
 }
 
 mmb_ctx_t *mmb_default_ctx(void);
@@ -1271,7 +1361,10 @@ void format_reads(std::string &out, FileBatch &fb, int lo, int hi, const mm_idx_
 		const char *qual = rec.qual.empty()? nullptr : rec.qual.c_str();
 		const int n_regs = fb.n_regs[i];
 		mm_reg1_t *regs = fb.regs[i];
-		if (n_regs > 0) {
+		if (opt->flag & MM_F_OUT_JUNC) { // --write-junc (map.c:601-607): junctions of the primary hits of MAPQ >= 10 instead of PAF / SAM
+			for (int j = 0; j < n_regs; ++j)
+				if (regs[j].id == regs[j].parent && regs[j].mapq >= 10) hl_write_junc(out, idx, fb.names[i], &regs[j]);
+		} else if (n_regs > 0) {
 			for (int j = 0; j < n_regs; ++j) {
 				const mm_reg1_t *rg = &regs[j];
 				if ((opt->flag & MM_F_NO_PRINT_2ND) && rg->id != rg->parent) continue;

@@ -141,6 +141,10 @@ struct ProfScope {
 
 // ---- device-side launchers (all asynchronous on ctx->stream) ----
 
+// map.cu / jump.cuh: K5 on n_hits descriptors (device), reads d_seq (nt4) and mi's device jump table; decisions to d_out
+void mmb_jump_device(mmb_ctx_t *ctx, const mm_idx_t *mi, const mm_mapopt_t *opt, int n_hits, const mmb_jump_hit_t *d_hits, const uint8_t *d_seq, mmb_jump_dec_t *d_out);
+bool mmb_jump_wanted(const mm_idx_t *mi, const mm_mapopt_t *opt, int qlen, const mm_reg1_t *r); // mm_jump_check of either end
+
 // ksw_extd2.cu: d_jobs/d_res are device arrays; query is a device byte array (nt4), target either bytes or 4-bit packed words.
 // h_jobs is the host copy (used for tiering). cigar ops go to d_cigar (capacity cigar_cap), *d_cigar_used counts them.
 void mmb_ksw_launch(mmb_ctx_t *ctx, const mmb_ksw_score_t *sc, int n_jobs, const mmb_ksw_job_t *h_jobs, const mmb_ksw_job_t *d_jobs,

@@ -232,17 +232,11 @@ extern "C" long peakrss(void) // misc.c:35-44
 	getrusage(RUSAGE_SELF, &r);
 	return r.ru_maxrss * 1024;
 }
-// split-index merging (main.c:511, --split-prefix) and jump annotations for short RNA-seq reads (main.c:473-478, -j / --pass1) are outside
-// the hot-path scope: the entry points exist so that main.c links unchanged; they refuse instead of pretending.
+// split-index merging (main.c:511, --split-prefix) is outside the hot-path scope: the entry point exists so that main.c links unchanged;
+// it refuses instead of pretending.
 extern "C" int mm_split_merge(int n_segs, const char **fn, const mm_mapopt_t *opt, int n_split_idx)
 {
 	(void)n_segs; (void)fn; (void)opt; (void)n_split_idx;
 	fprintf(stderr, "[ERROR] minimap2_b200: --split-prefix (multi-part index merging) is not supported\n");
-	return -1;
-}
-extern "C" int mm_idx_jjump_read(mm_idx_t *mi, const char *fn, int flag, int min_sc)
-{
-	(void)mi; (void)fn; (void)flag; (void)min_sc;
-	fprintf(stderr, "[ERROR] minimap2_b200: junction jump annotation (-j / --pass1, short RNA-seq reads) is not supported\n");
 	return -1;
 }

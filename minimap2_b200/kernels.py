@@ -103,3 +103,39 @@ def chain_rmq_batch(ctx, anchor_arrays, max_dist, max_dist_inner, bw, max_skip, 
         o = int(off[i])
         out.append((u[o:o + n_u[i]].copy(), ao[o:o + n_v[i]].copy()))
     return out
+
+
+class JumpHit(C.Structure):  # mmb_jump_hit_t (include/mm_b200.h)
+    _fields_ = [("rid", C.c_int32), ("rs", C.c_int32), ("re", C.c_int32), ("qs", C.c_int32), ("qe", C.c_int32), ("rev", C.c_int32),
+                ("qlen", C.c_int32), ("n_cigar", C.c_int32), ("q_off", C.c_int64), ("cig_first", C.c_uint32), ("cig_last", C.c_uint32)]
+
+
+class JumpSide(C.Structure):  # mmb_jump_side_t
+    _fields_ = [("act", C.c_int32), ("l", C.c_int32), ("off", C.c_int32), ("off2", C.c_int32), ("mm0", C.c_int32)]
+
+
+class JumpDec(C.Structure):  # mmb_jump_dec_t
+    _fields_ = [("side", JumpSide * 2)]
+
+
+def jump_batch(ctx, idx, map_opt, reads, hits, L=None):
+    """K5 (junction jumps) on the device. idx: mm_idx_t pointer with a jump table (mm_idx_jjump_read); map_opt: MapOpt (a, b,
+    jump_min_match); reads: list of bytes (ASCII); hits: list of dicts with read (index into reads), rid, rs, re, qs, qe, rev and cigar
+    (list of uint32 words). Returns one ((act, l, off, off2, mm0) left, (...) right) pair per hit. L: the library to call (default:
+    this package's)."""
+    off = np.zeros(len(reads) + 1, dtype=np.int64)
+    for i, s in enumerate(reads):
+        off[i + 1] = off[i] + len(s)
+    buf = np.frombuffer(b"".join(reads) + b"\0", dtype=np.uint8)
+    n = len(hits)
+    h = (JumpHit * max(n, 1))()
+    for i, x in enumerate(hits):
+        e = h[i]
+        e.rid, e.rs, e.re, e.qs, e.qe, e.rev = x["rid"], x["rs"], x["re"], x["qs"], x["qe"], x["rev"]
+        e.qlen, e.n_cigar, e.q_off = len(reads[x["read"]]), len(x["cigar"]), int(off[x["read"]])
+        e.cig_first, e.cig_last = x["cigar"][0], x["cigar"][-1]
+    out = (JumpDec * max(n, 1))()
+    ret = (L or lib()).mmb_jump_batch_host(C.c_void_p(ctx.h), idx, C.byref(map_opt), len(reads), C.c_void_p(buf.ctypes.data),
+                                    C.c_void_p(off.ctypes.data), n, h, out)
+    assert ret == 0, "mmb_jump_batch_host: the index has no jump table"
+    return [tuple((s.act, s.l, s.off, s.off2, s.mm0) for s in out[i].side) for i in range(n)]
