@@ -140,6 +140,18 @@ int mmb_chain_batch_host(mmb_ctx_t *ctx, const mmb_chain_par_t *par, int n_reads
  * par: max_dist_x = max_dist, max_dist_inner, bw, max_skip, rmq_size_cap, min_cnt, min_sc, chn_pen_gap, chn_pen_skip. */
 int mmb_chain_rmq_batch_host(mmb_ctx_t *ctx, const mmb_chain_par_t *par, int n_reads, const uint64_t *anchors_xy, const int64_t *a_off,
 							 int32_t *n_u, int32_t *n_v, uint64_t *u_out, uint64_t *a_out_xy);
+/* The long-join rescue (map.c:283-292): its selection rule and its mg_lchain_rmq parameters. max_skip, min_cnt, min_sc and the
+ * penalties are the first chainer's. */
+typedef struct {
+	int32_t bw_long, rescue_size;
+	float rescue_ratio;
+	int32_t max_dist, max_dist_inner, rmq_size_cap;
+} mmb_rescue_par_t;
+/* Same layout: the mapper's whole chaining stage. The first chainer (mg_lchain_dp, or mg_lchain_rmq when par->use_rmq) runs on
+ * every read, then the reads with more than one chain whose best chain passes the rescue test on qlen[i] are re-sorted and
+ * re-chained with mg_lchain_rmq at rp->bw_long. */
+int mmb_chain_rescue_batch_host(mmb_ctx_t *ctx, const mmb_chain_par_t *par, const mmb_rescue_par_t *rp, int n_reads, const uint64_t *anchors_xy,
+								const int64_t *a_off, const int32_t *qlen, int32_t *n_u, int32_t *n_v, uint64_t *u_out, uint64_t *a_out_xy);
 
 /* ---------------------------------------------------------------------------------------------------------
  * K4: per-hit tail of the alignment driver on the device   (replaces mm_append_cigar align.c:317-334, mm_fix_cigar

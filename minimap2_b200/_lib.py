@@ -35,6 +35,11 @@ class ChainPar(C.Structure):  # mmb_chain_par_t
                 ("use_rmq", C.c_int32), ("max_dist_inner", C.c_int32), ("rmq_size_cap", C.c_int32)]
 
 
+class RescuePar(C.Structure):  # mmb_rescue_par_t
+    _fields_ = [("bw_long", C.c_int32), ("rescue_size", C.c_int32), ("rescue_ratio", C.c_float),
+                ("max_dist", C.c_int32), ("max_dist_inner", C.c_int32), ("rmq_size_cap", C.c_int32)]
+
+
 def lib():
     global _lib
     if _lib is None:
@@ -65,6 +70,9 @@ def lib():
         L.mmb_chain_batch_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.mmb_chain_rmq_batch_host.restype = C.c_int
         L.mmb_chain_rmq_batch_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.mmb_chain_rescue_batch_host.restype = C.c_int
+        L.mmb_chain_rescue_batch_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 

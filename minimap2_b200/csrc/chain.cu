@@ -122,9 +122,12 @@ __global__ void __launch_bounds__(128) chain_fill_kernel(ChainArgs A)
 	if (max_dist_y < bw && !is_cdna) max_dist_y = bw;
 	// Pass 1 (all lanes, one anchor each): the start of anchor i's predecessor window has a closed form -- st is monotone
 	// in i in the reference (lchain.c:170-172), so st_i = max(lower_bound(x_i - max_dist_x within the same strand/contig),
-	// i - max_iter) -- found by binary search. An anchor with an empty window (st_i == i: the bulk of the seed hits, which
-	// are isolated) gets f = span, p = -1 and leaves max_ii = i behind, whatever came before; only the others need the
-	// sequential DP below. Their indices are compacted in order into `lst`.
+	// i - max_iter) -- found by binary search. An anchor with x_i - x_{i-1} > max_dist_x (the bulk of the seed hits, which
+	// are isolated) has no predecessor in range and is also too far from every earlier max_ii to keep it: it gets f = span,
+	// p = -1 and leaves max_ii = i behind, whatever came before (stv = -1 marks it). Every other anchor needs the sequential
+	// DP below, including those whose window only the max_iter cut emptied (st_i >= i: they still take the max_ii shortcut)
+	// and those whose window is empty because the previous anchor lies on another contig yet within max_dist_x in x.
+	// Their indices are compacted in order into `lst`.
 	int32_t *stv = (int32_t*)(A.z + off), *lst = (int32_t*)(A.b + off);
 	int32_t n_lst = 0;
 	for (int32_t i0 = 0; i0 < n; i0 += 32) {
@@ -132,14 +135,16 @@ __global__ void __launch_bounds__(128) chain_fill_kernel(ChainArgs A)
 		bool nontriv = false;
 		if (i < n) {
 			const m128 ai = a[i];
-			const uint64_t base = ai.x >> 32 << 32;
-			const uint64_t lo = ai.x - base > (uint64_t)(int64_t)max_dist_x? ai.x - (uint64_t)(int64_t)max_dist_x : base;
-			int32_t l = 0, h = i; // first j in [0, i] with a[j].x >= lo
-			while (l < h) { const int32_t m = (l + h) >> 1; if (a[m].x < lo) l = m + 1; else h = m; }
-			if (i - l > max_iter) l = i - max_iter;
-			stv[i] = l, t[i] = 0;
-			nontriv = l < i;
-			if (!nontriv) { const int32_t sp = (int32_t)(ai.y >> 32 & 0xff); f[i] = sp, p[i] = -1, v[i] = sp; }
+			t[i] = 0;
+			nontriv = i > 0 && ai.x - a[i - 1].x <= (uint64_t)(int64_t)max_dist_x;
+			if (nontriv) {
+				const uint64_t base = ai.x >> 32 << 32;
+				const uint64_t lo = ai.x - base > (uint64_t)(int64_t)max_dist_x? ai.x - (uint64_t)(int64_t)max_dist_x : base;
+				int32_t l = 0, h = i; // first j in [0, i] with a[j].x >= lo
+				while (l < h) { const int32_t m = (l + h) >> 1; if (a[m].x < lo) l = m + 1; else h = m; }
+				if (i - l > max_iter) l = i - max_iter; // lchain.c:173; st > i when max_iter < 0
+				stv[i] = l;
+			} else { const int32_t sp = (int32_t)(ai.y >> 32 & 0xff); f[i] = sp, p[i] = -1, v[i] = sp, stv[i] = -1; }
 		}
 		const unsigned m = __ballot_sync(full, nontriv);
 		if (nontriv) lst[n_lst + __popc(m & ((1u << lane) - 1))] = i;
@@ -151,8 +156,9 @@ __global__ void __launch_bounds__(128) chain_fill_kernel(ChainArgs A)
 		const int32_t i = lst[li];
 		const m128 ai = a[i];
 		const int32_t st = stv[i];
-		if (stv[i - 1] == i - 1) best_prev = i - 1; // the previous anchor was skipped: it reset max_ii to itself
-		int32_t max_f = (int32_t)(ai.y >> 32 & 0xff), max_j = -1, n_skip = 0, end_j = st - 1;
+		if (stv[i - 1] < 0) best_prev = i - 1; // the previous anchor was skipped: it reset max_ii to itself
+		// end_j: where the scan stopped; i - 1 when it never started (st > i after a negative max_iter's cut)
+		int32_t max_f = (int32_t)(ai.y >> 32 & 0xff), max_j = -1, n_skip = 0, end_j = min(st, i) - 1;
 		bool brk = false;
 		for (int32_t j_hi = i - 1; j_hi >= st && !brk; j_hi -= 32) {
 			const int32_t j = j_hi - lane;
@@ -541,6 +547,50 @@ void mmb_chain_rmq_primary_device(mmb_ctx_t *ctx, const mmb_chain_par_t *par, in
 	chain_rescue_kernel<<<(n_reads + 63) / 64, 64, 0, ctx->stream>>>(A, R);
 	MMB_CUDA_CHECK(cudaGetLastError());
 	++ctx->n_launch;
+}
+
+void mmb_chain_stage(mmb_ctx_t *ctx, const mmb_chain_par_t *par, const RescuePar *rp, int n_reads, const m128 *d_a, const int64_t *d_a_off,
+					 int64_t n_tot, int32_t *d_n_u, int32_t *d_n_v, uint64_t *d_u, m128 *d_a_out, int64_t *d_vo,
+					 DevBuf &scratch, DevBuf &scratch2, DevBuf &treebuf)
+{
+	if (par->use_rmq) mmb_chain_rmq_primary_device(ctx, par, n_reads, d_a, d_a_off, n_tot, d_n_u, d_n_v, d_u, d_a_out, scratch, scratch2, treebuf);
+	else mmb_chain_device(ctx, par, n_reads, d_a, d_a_off, n_tot, d_n_u, d_n_v, d_u, d_a_out, scratch, scratch2);
+	if (!rp || n_reads <= 0) return;
+	// the rescue's trees take 64 B per compacted anchor plus one node per read: read rd's start at tree_off[rd] + rd
+	mmb_widen_i32_async(ctx, d_n_v, n_reads, d_vo);
+	const int64_t tot_v = mmb_exclusive_scan_i64(ctx, d_vo, n_reads, true);
+	RescuePar R = *rp;
+	R.primary = 0, R.tree_off = d_vo;
+	mmb_chain_rescue_device(ctx, &R, n_reads, d_a_off, n_tot, d_n_u, d_n_v, d_u, d_a_out, scratch, scratch2, treebuf, tot_v);
+}
+
+extern "C" int mmb_chain_rescue_batch_host(mmb_ctx_t *ctx, const mmb_chain_par_t *par, const mmb_rescue_par_t *rp, int n_reads, const uint64_t *anchors_xy,
+										   const int64_t *a_off, const int32_t *qlen, int32_t *n_u, int32_t *n_v, uint64_t *u_out, uint64_t *a_out_xy)
+{
+	if (n_reads <= 0) return 0;
+	MMB_CUDA_CHECK(cudaSetDevice(ctx->device));
+	const int64_t n_tot = a_off[n_reads];
+	m128 *d_a = ctx->d_a.as<m128>((size_t)n_tot + 1);
+	int64_t *d_off = ctx->d_b.as<int64_t>((size_t)(n_reads + 1) * 2), *d_vo = d_off + (n_reads + 1);
+	int32_t *d_nu = ctx->d_c.as<int32_t>((size_t)n_reads * 3 + 3), *d_nv = d_nu + n_reads, *d_qlen = d_nv + n_reads;
+	uint64_t *d_u = ctx->d_d.as<uint64_t>((size_t)n_tot + 1);
+	m128 *d_ao = ctx->d_e.as<m128>((size_t)n_tot + 1);
+	MMB_CUDA_CHECK(cudaMemcpyAsync(d_a, anchors_xy, sizeof(m128) * n_tot, cudaMemcpyHostToDevice, ctx->stream));
+	MMB_CUDA_CHECK(cudaMemcpyAsync(d_off, a_off, sizeof(int64_t) * (n_reads + 1), cudaMemcpyHostToDevice, ctx->stream));
+	MMB_CUDA_CHECK(cudaMemcpyAsync(d_qlen, qlen, sizeof(int32_t) * n_reads, cudaMemcpyHostToDevice, ctx->stream));
+	RescuePar R;
+	memset(&R, 0, sizeof(R));
+	R.qlen = d_qlen, R.rescue_size = rp->rescue_size, R.rescue_ratio = rp->rescue_ratio;
+	R.max_dist = rp->max_dist, R.max_dist_inner = rp->max_dist_inner, R.bw = rp->bw_long, R.max_skip = par->max_skip;
+	R.rmq_size_cap = rp->rmq_size_cap, R.min_cnt = par->min_cnt, R.min_sc = par->min_sc;
+	R.pen_gap = par->chn_pen_gap, R.pen_skip = par->chn_pen_skip;
+	mmb_chain_stage(ctx, par, &R, n_reads, d_a, d_off, n_tot, d_nu, d_nv, d_u, d_ao, d_vo, ctx->d_f, ctx->d_g, ctx->d_h);
+	MMB_CUDA_CHECK(cudaMemcpyAsync(n_u, d_nu, sizeof(int32_t) * n_reads, cudaMemcpyDeviceToHost, ctx->stream));
+	MMB_CUDA_CHECK(cudaMemcpyAsync(n_v, d_nv, sizeof(int32_t) * n_reads, cudaMemcpyDeviceToHost, ctx->stream));
+	MMB_CUDA_CHECK(cudaMemcpyAsync(u_out, d_u, sizeof(uint64_t) * n_tot, cudaMemcpyDeviceToHost, ctx->stream));
+	MMB_CUDA_CHECK(cudaMemcpyAsync(a_out_xy, d_ao, sizeof(m128) * n_tot, cudaMemcpyDeviceToHost, ctx->stream));
+	MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+	return 0;
 }
 
 // Kernel-level entry for mg_lchain_rmq alone (lchain.c:251-357), HOST buffers. Used by the parity tests against the reference function.

@@ -210,12 +210,6 @@ __global__ void dust_filter_kernel(m128 *mz, const int64_t *mz_off, int32_t *n_m
 	n_mz[rd] = k;
 }
 
-__global__ void to_i64_kernel(const int32_t *a, int n, int64_t *b)
-{
-	int i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i < n) b[i] = a[i];
-}
-
 __global__ void copy_i64_kernel(const int64_t *a, int n, int64_t *b)
 {
 	int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -513,30 +507,25 @@ static void chain_batch(Batch &b, const MapPass &pass, GateHold &gate1)
 	int32_t *d_n_u = bb.n_u.as<int32_t>((size_t)n), *d_n_v = bb.n_v.as<int32_t>((size_t)n);
 	uint64_t *d_u = bb.u.as<uint64_t>((size_t)total_a + 4);
 	m128 *d_a_out = bb.a_out.as<m128>((size_t)total_a + 4);
-	if (opt->flag & MM_F_RMQ) { // map.c:275-276
+	if (opt->flag & MM_F_RMQ) // map.c:275-276
 		cp.use_rmq = 1, cp.max_dist_x = opt->max_gap, cp.max_dist_inner = opt->rmq_inner_dist, cp.rmq_size_cap = opt->rmq_size_cap;
-		mmb_chain_rmq_primary_device(ctx, &cp, n, S.a_sorted, d_a_off, total_a, d_n_u, d_n_v, d_u, d_a_out, bb.ch1, bb.ch2, bb.t1);
-	} else mmb_chain_device(ctx, &cp, n, S.a_sorted, d_a_off, total_a, d_n_u, d_n_v, d_u, d_a_out, bb.ch1, bb.ch2);
-	// dense copies for the host: offsets for u, a and mini_pos
-	int64_t *d_doff = bb.doff.as<int64_t>((size_t)(n + 1) * 3);
-	int64_t *d_uo = d_doff, *d_vo = d_doff + (n + 1), *d_mo = d_doff + 2 * (n + 1);
 	// long-join rescue (map.c:283-292): re-chain on the device with mg_lchain_rmq at bw_long
-	if (pass.rescue && opt->bw_long > opt->bw && (opt->flag & (MM_F_SPLICE | MM_F_SR | MM_F_NO_LJOIN)) == 0) {
-		to_i64_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_n_v, n, d_vo);
-		++ctx->n_launch;
-		const int64_t tv = mmb_exclusive_scan_i64(ctx, d_vo, n, true);
-		RescuePar rp;
-		rp.primary = 0;
+	RescuePar rp;
+	memset(&rp, 0, sizeof(rp));
+	const bool rescue = pass.rescue && opt->bw_long > opt->bw && (opt->flag & (MM_F_SPLICE | MM_F_SR | MM_F_NO_LJOIN)) == 0;
+	if (rescue) {
 		rp.qlen = b.d_qlen, rp.rescue_size = opt->rmq_rescue_size, rp.rescue_ratio = opt->rmq_rescue_ratio;
 		rp.max_dist = opt->max_gap, rp.max_dist_inner = opt->rmq_inner_dist, rp.bw = opt->bw_long, rp.max_skip = opt->max_chain_skip;
 		rp.rmq_size_cap = opt->rmq_size_cap, rp.min_cnt = opt->min_cnt, rp.min_sc = opt->min_chain_score;
-		rp.pen_gap = cp.chn_pen_gap, rp.pen_skip = cp.chn_pen_skip, rp.tree = nullptr, rp.tree_off = d_vo;
-		mmb_chain_rescue_device(ctx, &rp, n, d_a_off, total_a, d_n_u, d_n_v, d_u, d_a_out, bb.ch1, bb.ch2, bb.t1, tv);
+		rp.pen_gap = cp.chn_pen_gap, rp.pen_skip = cp.chn_pen_skip;
 	}
-	to_i64_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_n_u, n, d_uo);
-	to_i64_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(d_n_v, n, d_vo);
-	to_i64_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(S.n_keep, n, d_mo);
-	ctx->n_launch += 3;
+	// dense copies for the host: offsets for u, a and mini_pos
+	int64_t *d_doff = bb.doff.as<int64_t>((size_t)(n + 1) * 3);
+	int64_t *d_uo = d_doff, *d_vo = d_doff + (n + 1), *d_mo = d_doff + 2 * (n + 1);
+	mmb_chain_stage(ctx, &cp, rescue? &rp : nullptr, n, S.a_sorted, d_a_off, total_a, d_n_u, d_n_v, d_u, d_a_out, d_vo, bb.ch1, bb.ch2, bb.t1);
+	mmb_widen_i32_async(ctx, d_n_u, n, d_uo);
+	mmb_widen_i32_async(ctx, d_n_v, n, d_vo);
+	mmb_widen_i32_async(ctx, S.n_keep, n, d_mo);
 	const int64_t tot_u = mmb_exclusive_scan_i64(ctx, d_uo, n, true);
 	const int64_t tot_v = mmb_exclusive_scan_i64(ctx, d_vo, n, true);
 	const int64_t tot_m = mmb_exclusive_scan_i64(ctx, d_mo, n, true);

@@ -47,6 +47,11 @@ void mmb_chain_rmq_primary_device(mmb_ctx_t *ctx, const mmb_chain_par_t *par, in
 								  int32_t *d_n_u, int32_t *d_n_v, uint64_t *d_u, m128 *d_a_out, DevBuf &scratch, DevBuf &scratch2, DevBuf &treebuf);
 void mmb_chain_rescue_device(mmb_ctx_t *ctx, const RescuePar *rp, int n_reads, const int64_t *d_a_off, int64_t n_tot,
 							 int32_t *d_n_u, int32_t *d_n_v, uint64_t *d_u, m128 *d_a_out, DevBuf &scratch, DevBuf &scratch2, DevBuf &treebuf, int64_t tot_v);
+// The chaining stage of a batch (map.c:262-292): the first chainer (mmb_chain_rmq_primary_device when par->use_rmq, else
+// mmb_chain_device), then, when rp is given, the long-join rescue. d_vo (n_reads+1) receives the rescue's tree offsets.
+void mmb_chain_stage(mmb_ctx_t *ctx, const mmb_chain_par_t *par, const RescuePar *rp, int n_reads, const m128 *d_a, const int64_t *d_a_off,
+					 int64_t n_tot, int32_t *d_n_u, int32_t *d_n_v, uint64_t *d_u, m128 *d_a_out, int64_t *d_vo,
+					 DevBuf &scratch, DevBuf &scratch2, DevBuf &treebuf);
 
 // ---- K4 (finalize.cu): CIGAR assembly + mm_fix_cigar + mm_update_extra of finished hits on the device (align.c:105-181,254-334) ----
 struct FinJobRef { const uint32_t *cig; uint32_t n, pad; }; // one ksw2 result: its CIGAR in the device arena of the wave that ran it

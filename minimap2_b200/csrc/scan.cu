@@ -62,7 +62,20 @@ __global__ void stk_len_kernel(const int64_t *a_off, int n_reads, int64_t *stk_o
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i < n_reads) stk_off[i] = mmx_rs_stack_len(a_off[i + 1] - a_off[i]);
 }
+
+__global__ void widen_i32_kernel(const int32_t *a, int n, int64_t *b)
+{
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) b[i] = a[i];
+}
 } // namespace
+
+void mmb_widen_i32_async(mmb_ctx_t *ctx, const int32_t *src, int n, int64_t *d)
+{
+	if (n <= 0) return;
+	widen_i32_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(src, n, d);
+	++ctx->n_launch;
+}
 
 void mmb_exclusive_scan_i64_async(mmb_ctx_t *ctx, int64_t *d, int64_t n)
 {

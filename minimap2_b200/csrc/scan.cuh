@@ -7,6 +7,8 @@
 int64_t mmb_exclusive_scan_i64(mmb_ctx_t *ctx, int64_t *d, int64_t n, bool with_total);
 // Same without returning/synchronising (total written to d[n]).
 void mmb_exclusive_scan_i64_async(mmb_ctx_t *ctx, int64_t *d, int64_t n);
+// d[i] = src[i] for i < n (asynchronous)
+void mmb_widen_i32_async(mmb_ctx_t *ctx, const int32_t *src, int n, int64_t *d);
 
 // Stacks of mmx_rs_sort for every read of a batch with n_tot anchors in all (which reads will need one is not known in advance).
 // Reserves head_bytes for the caller at the start of buf, then n_reads+1 per-read stack offsets, then the stacks; fills the offsets on

@@ -1,7 +1,7 @@
 """Kernel-level host-buffer entry points (the C-ABI calls in include/mm_b200.h), used by the parity tests."""
 import ctypes as C
 import numpy as np
-from ._lib import lib, KswJob, KswRes, KswScore, ChainPar
+from ._lib import lib, KswJob, KswRes, KswScore, ChainPar, RescuePar
 
 
 def make_score(mat, q, e, q2, e2, noncan=0, junc_bonus=0, junc_pen=0, zd_skip=0):
@@ -65,8 +65,8 @@ def sketch_batch(ctx, seqs, w, k, is_hpc=0, rid0=0):
     return res
 
 
-def chain_batch(ctx, anchor_arrays, max_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt, min_sc, pen_gap, pen_skip=0.0, is_cdna=0, n_seg=1):
-    """anchor_arrays: list of (n_i,2) uint64 arrays sorted by x. Returns list of (u, a) like mg_lchain_dp."""
+def _chain_io(anchor_arrays):
+    """concatenated anchors, offsets and output buffers of the chaining entries"""
     n = len(anchor_arrays)
     off = np.zeros(n + 1, dtype=np.int64)
     for i, a in enumerate(anchor_arrays):
@@ -74,35 +74,41 @@ def chain_batch(ctx, anchor_arrays, max_dist_x, max_dist_y, bw, max_skip, max_it
     tot = int(off[-1])
     cat = np.concatenate([np.asarray(a, dtype=np.uint64).reshape(-1, 2) for a in anchor_arrays]) if tot else np.zeros((0, 2), dtype=np.uint64)
     cat = np.ascontiguousarray(cat)
-    par = ChainPar(max_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt, min_sc, pen_gap, pen_skip, is_cdna, n_seg, 0, 0, 0)
     n_u = np.zeros(n, dtype=np.int32); n_v = np.zeros(n, dtype=np.int32)
     u = np.zeros(tot + 1, dtype=np.uint64); ao = np.zeros((tot + 1, 2), dtype=np.uint64)
-    lib().mmb_chain_batch_host(ctx.h, C.byref(par), n, cat.ctypes.data, off.ctypes.data, n_u.ctypes.data, n_v.ctypes.data, u.ctypes.data, ao.ctypes.data)
-    out = []
-    for i in range(n):
-        o = int(off[i])
-        out.append((u[o:o + n_u[i]].copy(), ao[o:o + n_v[i]].copy()))
-    return out
+    return off, cat, n_u, n_v, u, ao
+
+
+def _chain_out(off, n_u, n_v, u, ao):
+    return [(u[int(off[i]):int(off[i]) + n_u[i]].copy(), ao[int(off[i]):int(off[i]) + n_v[i]].copy()) for i in range(len(n_u))]
+
+
+def chain_batch(ctx, anchor_arrays, max_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt, min_sc, pen_gap, pen_skip=0.0, is_cdna=0, n_seg=1):
+    """anchor_arrays: list of (n_i,2) uint64 arrays sorted by x. Returns list of (u, a) like mg_lchain_dp."""
+    off, cat, n_u, n_v, u, ao = _chain_io(anchor_arrays)
+    par = ChainPar(max_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt, min_sc, pen_gap, pen_skip, is_cdna, n_seg, 0, 0, 0)
+    lib().mmb_chain_batch_host(ctx.h, C.byref(par), len(n_u), cat.ctypes.data, off.ctypes.data, n_u.ctypes.data, n_v.ctypes.data, u.ctypes.data, ao.ctypes.data)
+    return _chain_out(off, n_u, n_v, u, ao)
 
 
 def chain_rmq_batch(ctx, anchor_arrays, max_dist, max_dist_inner, bw, max_skip, cap, min_cnt, min_sc, pen_gap, pen_skip=0.0):
     """mg_lchain_rmq on every read (anchors sorted by x). Returns list of (u, a)."""
-    n = len(anchor_arrays)
-    off = np.zeros(n + 1, dtype=np.int64)
-    for i, a in enumerate(anchor_arrays):
-        off[i + 1] = off[i] + len(a)
-    tot = int(off[-1])
-    cat = np.concatenate([np.asarray(a, dtype=np.uint64).reshape(-1, 2) for a in anchor_arrays]) if tot else np.zeros((0, 2), dtype=np.uint64)
-    cat = np.ascontiguousarray(cat)
+    off, cat, n_u, n_v, u, ao = _chain_io(anchor_arrays)
     par = ChainPar(max_dist, max_dist, bw, max_skip, 5000, min_cnt, min_sc, pen_gap, pen_skip, 0, 1, 1, max_dist_inner, cap)
-    n_u = np.zeros(n, dtype=np.int32); n_v = np.zeros(n, dtype=np.int32)
-    u = np.zeros(tot + 1, dtype=np.uint64); ao = np.zeros((tot + 1, 2), dtype=np.uint64)
-    lib().mmb_chain_rmq_batch_host(ctx.h, C.byref(par), n, cat.ctypes.data, off.ctypes.data, n_u.ctypes.data, n_v.ctypes.data, u.ctypes.data, ao.ctypes.data)
-    out = []
-    for i in range(n):
-        o = int(off[i])
-        out.append((u[o:o + n_u[i]].copy(), ao[o:o + n_v[i]].copy()))
-    return out
+    lib().mmb_chain_rmq_batch_host(ctx.h, C.byref(par), len(n_u), cat.ctypes.data, off.ctypes.data, n_u.ctypes.data, n_v.ctypes.data, u.ctypes.data, ao.ctypes.data)
+    return _chain_out(off, n_u, n_v, u, ao)
+
+
+def chain_rescue_batch(ctx, anchor_arrays, qlens, par, rescue):
+    """The mapper's chaining stage (map.c:262-292) on every read: the first chainer that par (a ChainPar; use_rmq selects
+    mg_lchain_rmq) describes, then the long-join rescue (a RescuePar) of the reads it selects by their query length qlens[i].
+    Returns list of (u, a)."""
+    off, cat, n_u, n_v, u, ao = _chain_io(anchor_arrays)
+    ql = np.ascontiguousarray(qlens, dtype=np.int32)
+    assert len(ql) == len(n_u)
+    lib().mmb_chain_rescue_batch_host(ctx.h, C.byref(par), C.byref(rescue), len(n_u), cat.ctypes.data, off.ctypes.data, ql.ctypes.data,
+                                      n_u.ctypes.data, n_v.ctypes.data, u.ctypes.data, ao.ctypes.data)
+    return _chain_out(off, n_u, n_v, u, ao)
 
 
 class JumpHit(C.Structure):  # mmb_jump_hit_t (include/mm_b200.h)

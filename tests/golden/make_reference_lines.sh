@@ -11,7 +11,7 @@ cd "$(dirname "$0")/../.."
 out=${TMPDIR:-/tmp}/reference_lines.$$.json
 rm -f "$out" "$out.values.json"
 MM2_RECORD_REFERENCE=$out python -m pytest -q tests/test_emu_e2e.py tests/test_emu_api.py tests/test_oracle_seed.py \
-    tests/test_gpu_e2e.py tests/test_gpu_zz_splice.py tests/test_gpuext_options.py
+    tests/test_gpu_e2e.py tests/test_gpu_zz_splice.py tests/test_gpuext_options.py tests/test_gpu_chain_cli.py
 mv "$out" tests/golden/expected/reference_lines.json
 mv "$out.values.json" tests/golden/expected/reference_values.json
 oracle/_ref/minimap2 -t 2 -d tests/golden/data/MT-human.mmi tests/golden/data/MT-human.fa

@@ -233,6 +233,12 @@ def _multipart_inputs(d):
     return ["-c", "-I", "4k", "--paf-no-hit", rf, qf]
 
 
+# chaining options at their edges: every DP window emptied by the iteration cut, no skipped predecessor allowed, a skip penalty, and
+# an -r pair under which the long-join rescue re-chains the read (the reference's output differs with --no-long-join)
+CHAIN_OPTS = {"chain_iter0": ["-c", "--max-chain-iter", "0"], "chain_skip0": ["--max-chain-skip", "0"],
+              "chain_skip_scale": ["-c", "--chain-skip-scale", "1"], "long_join": ["-c", "-r", "20,5000"]}
+
+
 @pytest.fixture(scope="module")
 def emu_runs(emu_cli, tmp_path_factory):
     """Every emulated CLI run of this module, started together (6 at a time): the emulator spends most of its time in thread
@@ -260,6 +266,8 @@ def emu_runs(emu_cli, tmp_path_factory):
     jobs["sdust"] = (_sdust_inputs(d), d, True)
     jobs["waves"] = (_many_waves_inputs(d), d, True)
     jobs["multipart"] = (_multipart_inputs(d), d, True)
+    for name, opt in CHAIN_OPTS.items():
+        jobs[name] = (["-x", "map-ont"] + opt + ["x3s-ref.fa", "x3s-qry.fa"], data, True)
 
     def one(item):
         name, (args, cwd, with_ref), more_env = item[0], item[1][:3], (item[1][3] if len(item[1]) > 3 else {})
@@ -337,6 +345,17 @@ def test_emulated_high_occurrence_seed_selection_matches_reference(emu_runs):
     O.assert_matches_reference(r["out"], r["ref"])
     assert len(r["ref"]) >= 3
     assert any("rl:i:" in l and "rl:i:0" not in l for l in r["out"])  # the selection really masked something
+
+
+@pytest.mark.parametrize("name", sorted(CHAIN_OPTS))
+def test_emulated_chain_options_match_reference(emu_runs, name):
+    r = emu_runs[name]
+    assert r["rc"] == 0, r["err"]
+    O.assert_matches_reference(r["out"], r["ref"])
+    assert len(r["ref"]) >= 1
+    if name == "long_join":
+        args = ["-x", "map-ont"] + CHAIN_OPTS[name] + ["--no-long-join", "x3s-ref.fa", "x3s-qry.fa"]
+        assert O.reference_lines(args, os.path.join(GOLD, "data")).all != r["ref"].all  # the rescue changes this output
 
 
 @pytest.mark.parametrize("preset", ["asm5", "asm20"])
