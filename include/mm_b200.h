@@ -242,6 +242,10 @@ typedef struct {
 void mmb_idx_export(const mm_idx_t *mi, mmb_idx_desc_t *d);
 mm_idx_t *mmb_idx_adopt(const mmb_idx_desc_t *d, const char **names, const uint32_t *lens, const uint32_t *cnt_sorted_dev);
 const void *mmb_idx_cnt_sorted(const mm_idx_t *mi, uint64_t *bytes); /* sorted occurrence counts (mm_idx_cal_max_occ, index.c:158) */
+/* Kernel-level probe of the device index for tests: one thread per key looks it up in the device hash table with the seeding kernels'
+ * lookup (mm_idx_get, index.c:93-110) and gathers its occurrences. cnt[i]: occurrences of keys[i] (0: absent); occ_off[n+1]: where
+ * they start in occ (prefix sums of cnt); occ receives the first occ_cap of them. Returns the total. */
+int64_t mmb_idx_lookup_host(const mm_idx_t *mi, int64_t n, const uint64_t *keys, uint32_t *cnt, uint64_t *occ, int64_t occ_cap, int64_t *occ_off);
 
 /* K2a/K2b as one stage for kernel-level tests: sketch -> mm_seed_mz_flt -> mm_idx_get -> mm_seed_select -> collect_seed_hits incl.
  * radix_sort_128x (seed.c:5-132, map.c:59-72,168-204) of a batch of reads against a device-resident index. See csrc/map.cu. */

@@ -73,6 +73,8 @@ def lib():
         L.mmb_chain_rescue_batch_host.restype = C.c_int
         L.mmb_chain_rescue_batch_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.mmb_idx_lookup_host.restype = C.c_int64
+        L.mmb_idx_lookup_host.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
         _lib = L
     return _lib
 

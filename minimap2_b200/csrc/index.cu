@@ -841,3 +841,57 @@ extern "C" const void *mmb_idx_cnt_sorted(const mm_idx_t *mi, uint64_t *bytes)
 	*bytes = 4ull * (uint64_t)(mi->B->n_keys + 1);
 	return mi->B->d_cnt_sorted;
 }
+
+// ---------------------------------------------------------------------------------------------------------
+// Kernel-level probe of the device table (tests): the lookup the seeding kernels do, key by key
+// ---------------------------------------------------------------------------------------------------------
+namespace {
+
+__global__ void idx_probe_kernel(DevIndexView ix, const uint64_t *keys, int64_t n, int64_t *cnt, uint64_t *src)
+{
+	const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	uint64_t off;
+	cnt[i] = idx_get_dev(ix, keys[i], &off);
+	src[i] = off;
+}
+
+__global__ void idx_gather_kernel(DevIndexView ix, int64_t n, const int64_t *dst, const uint64_t *src, int64_t cap, uint64_t *occ)
+{
+	const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	for (int64_t j = dst[i], o = (int64_t)src[i]; j < dst[i + 1] && j < cap; ++j, ++o) occ[j] = ix.pos[o];
+}
+
+} // namespace
+
+extern "C" int64_t mmb_idx_lookup_host(const mm_idx_t *mi, int64_t n, const uint64_t *keys, uint32_t *cnt, uint64_t *occ, int64_t occ_cap, int64_t *occ_off)
+{
+	mm_idx_bucket_s *B = mi->B;
+	mmb_ctx_t *ctx = B->ctx;
+	MMB_CUDA_CHECK(cudaSetDevice(ctx->device));
+	if (n <= 0) { occ_off[0] = 0; return 0; }
+	uint64_t *d_keys, *d_src, *d_occ = nullptr;
+	int64_t *d_off;
+	MMB_CUDA_CHECK(cudaMalloc(&d_keys, 8 * (size_t)n));
+	MMB_CUDA_CHECK(cudaMalloc(&d_src, 8 * (size_t)n));
+	MMB_CUDA_CHECK(cudaMalloc(&d_off, 8 * (size_t)(n + 1)));
+	MMB_CUDA_CHECK(cudaMemcpy(d_keys, keys, 8 * (size_t)n, cudaMemcpyHostToDevice));
+	const DevIndexView ix = B->view(mi);
+	const unsigned grid = (unsigned)((n + 255) / 256);
+	idx_probe_kernel<<<grid, 256, 0, ctx->stream>>>(ix, d_keys, n, d_off, d_src);
+	MMB_CUDA_CHECK(cudaGetLastError());
+	const int64_t total = mmb_exclusive_scan_i64(ctx, d_off, n, true); // counts -> occurrence offsets, d_off[n] = total
+	if (total > 0 && occ_cap > 0) {
+		MMB_CUDA_CHECK(cudaMalloc(&d_occ, 8 * (size_t)std::min(total, occ_cap)));
+		idx_gather_kernel<<<grid, 256, 0, ctx->stream>>>(ix, n, d_off, d_src, occ_cap, d_occ);
+		MMB_CUDA_CHECK(cudaGetLastError());
+		MMB_CUDA_CHECK(cudaMemcpyAsync(occ, d_occ, 8 * (size_t)std::min(total, occ_cap), cudaMemcpyDeviceToHost, ctx->stream));
+	}
+	MMB_CUDA_CHECK(cudaMemcpyAsync(occ_off, d_off, 8 * (size_t)(n + 1), cudaMemcpyDeviceToHost, ctx->stream));
+	MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+	for (int64_t i = 0; i < n; ++i) cnt[i] = (uint32_t)(occ_off[i + 1] - occ_off[i]);
+	MMB_CUDA_CHECK(cudaFree(d_keys)); MMB_CUDA_CHECK(cudaFree(d_src)); MMB_CUDA_CHECK(cudaFree(d_off));
+	if (d_occ) MMB_CUDA_CHECK(cudaFree(d_occ));
+	return total;
+}

@@ -111,6 +111,24 @@ def chain_rescue_batch(ctx, anchor_arrays, qlens, par, rescue):
     return _chain_out(off, n_u, n_v, u, ao)
 
 
+def idx_lookup(idx, keys, L=None):
+    """The device hash table of idx (an mm_idx_t pointer) probed for every key, as the seeding kernels probe it. Returns (cnt, occ_off,
+    occ): occurrences of keys[i] (0: absent) and their words occ[occ_off[i]:occ_off[i + 1]], in stored order. L: the library to call
+    (default: this package's)."""
+    L = L or lib()
+    keys = np.ascontiguousarray(keys, dtype=np.uint64)
+    n = len(keys)
+    cnt, occ_off = np.zeros(max(n, 1), dtype=np.uint32), np.zeros(n + 1, dtype=np.int64)
+    occ = np.zeros(1, dtype=np.uint64)
+    for _ in range(2):  # the second call when the first capacity was too small
+        tot = L.mmb_idx_lookup_host(C.c_void_p(idx), C.c_int64(n), C.c_void_p(keys.ctypes.data), C.c_void_p(cnt.ctypes.data),
+                                    C.c_void_p(occ.ctypes.data), C.c_int64(len(occ)), C.c_void_p(occ_off.ctypes.data))
+        if tot <= len(occ):
+            break
+        occ = np.zeros(tot, dtype=np.uint64)
+    return cnt[:n], occ_off, occ[:tot]
+
+
 class JumpHit(C.Structure):  # mmb_jump_hit_t (include/mm_b200.h)
     _fields_ = [("rid", C.c_int32), ("rs", C.c_int32), ("re", C.c_int32), ("qs", C.c_int32), ("qe", C.c_int32), ("rev", C.c_int32),
                 ("qlen", C.c_int32), ("n_cigar", C.c_int32), ("q_off", C.c_int64), ("cig_first", C.c_uint32), ("cig_last", C.c_uint32)]

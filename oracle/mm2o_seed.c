@@ -81,6 +81,12 @@ const uint64_t *mm2o_idx_get(const mm2o_idx_t *mi, uint64_t minier, int *n) /* i
 	return 0;
 }
 
+int64_t mm2o_idx_keys(const mm2o_idx_t *mi, const uint64_t **keys, const int64_t **start, const uint64_t **pos)
+{
+	*keys = mi->key, *start = mi->start, *pos = mi->pos;
+	return mi->n_keys;
+}
+
 typedef struct { uint32_t n, q_pos; uint32_t q_span:8, flt:1, seg_id:8, is_tandem:1; const uint64_t *cr; } seed_t; /* mmpriv.h:45-51 */
 
 static void heap_down(size_t i, size_t n, uint64_t *l) /* ksort.h:44-56 with '<' */

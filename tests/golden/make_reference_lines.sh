@@ -11,8 +11,12 @@ cd "$(dirname "$0")/../.."
 out=${TMPDIR:-/tmp}/reference_lines.$$.json
 rm -f "$out" "$out.values.json"
 MM2_RECORD_REFERENCE=$out python -m pytest -q tests/test_emu_e2e.py tests/test_emu_api.py tests/test_oracle_seed.py \
-    tests/test_gpu_e2e.py tests/test_gpu_zz_splice.py tests/test_gpuext_options.py tests/test_gpu_chain_cli.py
+    tests/test_gpu_e2e.py tests/test_gpu_zz_splice.py tests/test_gpuext_options.py tests/test_gpu_chain_cli.py tests/test_index_cases_vs_ref.py tests/test_gpu_index_cli.py
 mv "$out" tests/golden/expected/reference_lines.json
 mv "$out.values.json" tests/golden/expected/reference_values.json
 oracle/_ref/minimap2 -t 2 -d tests/golden/data/MT-human.mmi tests/golden/data/MT-human.fa
 gzip -9 -n -f tests/golden/data/MT-human.mmi
+# an HPC index and an even-k index with b = 2k < 14 (tests/index_cases.py: REF_MMI)
+oracle/_ref/minimap2 -t 2 -H -w 10 -k 19 -d tests/golden/data/MT-human.H.w10k19.mmi tests/golden/data/MT-human.fa
+oracle/_ref/minimap2 -t 2 -w 4 -k 6 -d tests/golden/data/MT-human.w4k6.mmi tests/golden/data/MT-human.fa
+gzip -9 -n -f tests/golden/data/MT-human.H.w10k19.mmi tests/golden/data/MT-human.w4k6.mmi

@@ -36,14 +36,14 @@ def device_seeds(L, ctx, mi, reads, flag, mid_occ, q_occ_frac, max_max_occ, occ_
     return out
 
 
-def check_case(L, ctx, contigs, reads, w=10, k=15, flag=0, mid_occ=10, q_occ_frac=0.01, max_max_occ=4095, occ_dist=500):
+def check_case(L, ctx, contigs, reads, w=10, k=15, flag=0, mid_occ=10, q_occ_frac=0.01, max_max_occ=4095, occ_dist=500, is_hpc=0):
     names = ["chr%d" % i for i in range(len(contigs))]
     seqs = [bytes(c) for c in contigs]
     arr = (C.c_char_p * len(seqs))(*seqs); nm = (C.c_char_p * len(seqs))(*[x.encode() for x in names])
-    mi = L.mm_idx_str(w, k, 0, 14, len(seqs), arr, nm)
+    mi = L.mm_idx_str(w, k, is_hpc, 14, len(seqs), arr, nm)
     reads = [bytes(r) for r in reads]
     got = device_seeds(L, ctx, mi, reads, flag, mid_occ, q_occ_frac, max_max_occ, occ_dist)
-    idx = O.OracleIndex(seqs, names, w, k)
+    idx = O.OracleIndex(seqs, names, w, k, is_hpc)
     stats = dict(anchors=0, ties=0, big=0, wide=0)
     for i, s in enumerate(reads):
         ea, erep, emp = idx.anchors(s, flag=flag, mid_occ=mid_occ, q_occ_frac=q_occ_frac, max_max_occ=max_max_occ, occ_dist=occ_dist) if len(s) else (np.zeros((0, 2), dtype=np.uint64), 0, np.zeros(0, dtype=np.uint64))

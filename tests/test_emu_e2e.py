@@ -7,6 +7,7 @@ import subprocess
 import sys
 import pytest
 import oracle_lib as O
+import index_cases as IC
 
 sys.path.insert(0, os.path.join(O.ROOT, "tests", "cuda_emu"))
 GOLD = os.path.join(O.ROOT, "tests", "golden")
@@ -239,6 +240,10 @@ CHAIN_OPTS = {"chain_iter0": ["-c", "--max-chain-iter", "0"], "chain_skip0": ["-
               "chain_skip_scale": ["-c", "--chain-skip-scale", "1"], "long_join": ["-c", "-r", "20,5000"]}
 
 
+# a subset of tests/test_gpu_index_cli.py: an HPC preset, -H, and even k (the sketch_kernel build and query sketch)
+INDEX_LINES = {"map_pb": 0, "hpc_k15": 3, "even_k14": 4}
+
+
 @pytest.fixture(scope="module")
 def emu_runs(emu_cli, tmp_path_factory):
     """Every emulated CLI run of this module, started together (6 at a time): the emulator spends most of its time in thread
@@ -268,6 +273,9 @@ def emu_runs(emu_cli, tmp_path_factory):
     jobs["multipart"] = (_multipart_inputs(d), d, True)
     for name, opt in CHAIN_OPTS.items():
         jobs[name] = (["-x", "map-ont"] + opt + ["x3s-ref.fa", "x3s-qry.fa"], data, True)
+    lines = IC.cli_lines(*IC.cli_inputs(d, "hpc", 20_000, 4, 23))
+    for name, i in INDEX_LINES.items():
+        jobs[name] = (lines[i], d, True)
 
     def one(item):
         name, (args, cwd, with_ref), more_env = item[0], item[1][:3], (item[1][3] if len(item[1]) > 3 else {})
@@ -429,6 +437,15 @@ def test_emulated_cli_edge_cases_match_reference(emu_runs, name, n_min):
     assert r["rc"] == 0, r["err"]
     O.assert_matches_reference(r["out"], r["ref"])
     assert len(r["ref"]) >= n_min
+
+
+@pytest.mark.parametrize("name", sorted(INDEX_LINES))
+def test_emulated_index_options_match_reference(emu_runs, name):
+    """mapping with HPC and even-k indexes on homopolymer-rich inputs (tests/index_cases.py:cli_inputs)"""
+    r = emu_runs[name]
+    assert r["rc"] == 0, r["err"]
+    O.assert_matches_reference(r["out"], r["ref"])
+    assert len(r["ref"]) >= 3
 
 
 def test_mmi_files_are_interchangeable(emu_cli, tmp_path):
