@@ -248,7 +248,8 @@ const void *mmb_idx_cnt_sorted(const mm_idx_t *mi, uint64_t *bytes); /* sorted o
 int64_t mmb_idx_lookup_host(const mm_idx_t *mi, int64_t n, const uint64_t *keys, uint32_t *cnt, uint64_t *occ, int64_t occ_cap, int64_t *occ_off);
 
 /* K2a/K2b as one stage for kernel-level tests: sketch -> mm_seed_mz_flt -> mm_idx_get -> mm_seed_select -> collect_seed_hits incl.
- * radix_sort_128x (seed.c:5-132, map.c:59-72,168-204) of a batch of reads against a device-resident index. See csrc/map.cu. */
+ * radix_sort_128x (seed.c:5-132, map.c:59-72,168-204) of a batch of reads against a device-resident index. With MM_F_HEAP_SORT in
+ * flag the anchors come in the order of collect_seed_hits_heap (map.c:102-166) instead. See csrc/map.cu. */
 int64_t mmb_seed_batch_host(mmb_ctx_t *ctx, const mm_idx_t *mi, int n_reads, const char *seqs, const int64_t *off, int64_t flag, int mid_occ,
 							float q_occ_frac, int max_max_occ, int occ_dist, int64_t *a_off_out, int32_t *rep_len_out, int32_t *n_mini_out,
 							uint64_t *anchors_xy, int64_t a_cap, uint64_t *mini_pos, int64_t mp_cap);

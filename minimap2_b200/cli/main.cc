@@ -38,6 +38,7 @@ static struct option long_options[] = {
 	{ "no-self", no_argument, 0, 'D' }, { "max-chain-skip", required_argument, 0, 307 }, { "min-dp-len", required_argument, 0, 308 },
 	{ "splice", no_argument, 0, 310 }, { "no-long-join", no_argument, 0, 312 }, { "secondary", required_argument, 0, 315 },
 	{ "cs", optional_argument, 0, 316 }, { "end-bonus", required_argument, 0, 317 }, { "for-only", no_argument, 0, 322 }, { "qstrand", no_argument, 0, 348 },
+	{ "heap-sort", required_argument, 0, 324 },
 	{ "rev-only", no_argument, 0, 323 }, { "all-chain", no_argument, 0, 'P' }, { "dual", required_argument, 0, 326 },
 	{ "max-clip-ratio", required_argument, 0, 327 }, { "min-occ-floor", required_argument, 0, 328 }, { "MD", no_argument, 0, 329 },
 	{ "score-N", required_argument, 0, 331 }, { "eqx", no_argument, 0, 332 }, { "paf-no-hit", no_argument, 0, 333 },
@@ -172,6 +173,7 @@ int main(int argc, char *argv[])
 		else if (c == 356) opt.rmq_inner_dist = (int)parse_num(optarg);
 		else if (c == 315) yes_or_no(&opt, MM_F_NO_PRINT_2ND, "secondary", optarg, 0);
 		else if (c == 326) yes_or_no(&opt, MM_F_NO_DUAL, "dual", optarg, 0);
+		else if (c == 324) yes_or_no(&opt, MM_F_HEAP_SORT, "heap-sort", optarg, 1);
 		else if (c == 316) {
 			opt.flag |= MM_F_OUT_CS | MM_F_CIGAR;
 			if (optarg == 0 || strcmp(optarg, "short") == 0) opt.flag &= ~MM_F_OUT_CS_LONG;

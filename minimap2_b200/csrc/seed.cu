@@ -15,6 +15,8 @@
 //   sort_block_kernel  1 CTA / read         bitonic sort of (x, index): the radix kernels' fallback for keys varying in > 33 bits
 //   sort_exact_smem    1 warp / read        exact emulation of the reference's unstable in-place MSD radix sort for tie reads
 //   sort_exact_kernel  1 thread / read      the same in global memory (mmx_rs_sort) for reads too large for sort_exact_smem
+//   heap_merge_kernel  1 thread / read      heap mode (MM_F_HEAP_SORT) instead of the two above: replay of the reference's heap merge
+//                                           (collect_seed_hits_heap) for the reads with equal keys and the oversize reads
 #include "index.h"
 #include "mm_algo.cuh"
 #include "scan.cuh"
@@ -356,6 +358,30 @@ __global__ void __launch_bounds__(128) skip_offsets_kernel(SeedArgs A)
 	A.n_a[rd] = run;
 }
 
+// One anchor of occurrence r of seed q (query minimizer q, seed-list word e: tandem flag in bit 31), as collect_seed_hits writes it
+// (map.c:182-197). qstrand selects the query-strand formula for reverse hits; the heap merge never uses it (map.c:134-136).
+__device__ __forceinline__ m128 make_anchor(const SeedArgs &A, uint64_t r, m128 q, uint32_t e, bool is_self, int qlen, bool qstrand)
+{
+	const uint32_t q_pos = (uint32_t)q.y, q_span = (uint32_t)(q.x & 0xff), seg_id = (uint32_t)(q.y >> 32);
+	const int32_t rpos = (int32_t)((uint32_t)r >> 1);
+	m128 p;
+	if ((r & 1) == (q_pos & 1)) {
+		p.x = (r & 0xffffffff00000000ULL) | (uint32_t)rpos;
+		p.y = (uint64_t)q_span << 32 | q_pos >> 1;
+	} else if (!qstrand) {
+		p.x = 1ULL << 63 | (r & 0xffffffff00000000ULL) | (uint32_t)rpos;
+		p.y = (uint64_t)q_span << 32 | (uint32_t)(qlen - ((int32_t)(q_pos >> 1) + 1 - (int32_t)q_span) - 1);
+	} else {
+		const int32_t len = (int32_t)A.ix.seq_len[r >> 32];
+		p.x = 1ULL << 63 | (r & 0xffffffff00000000ULL) | (uint32_t)(len - (rpos + 1 - (int32_t)q_span) - 1);
+		p.y = (uint64_t)q_span << 32 | q_pos >> 1;
+	}
+	p.y |= (uint64_t)seg_id << MMX_SEED_SEG_SHIFT;
+	if (e >> 31) p.y |= MMX_SEED_TANDEM;
+	if (is_self) p.y |= MMX_SEED_SELF;
+	return p;
+}
+
 __global__ void __launch_bounds__(256) expand_kernel(SeedArgs A, int64_t total) // map.c:176-199
 {
 	const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -366,34 +392,19 @@ __global__ void __launch_bounds__(256) expand_kernel(SeedArgs A, int64_t total) 
 	if (k >= A.n_keep[rd]) return;
 	const uint32_t e = A.k_idx[t], mi = e & 0x7fffffffu;
 	const m128 q = A.mz[base + mi];
-	const uint32_t q_pos = (uint32_t)q.y, q_span = (uint32_t)(q.x & 0xff), seg_id = (uint32_t)(q.y >> 32);
+	const uint32_t q_pos = (uint32_t)q.y;
 	const uint32_t n = A.s_n[base + mi];
 	const uint64_t *cr = A.ix.pos + A.s_off[base + mi];
 	m128 *a = A.a + A.a_off[rd] + A.k_aoff[t];
 	const int qlen = A.qlen[rd];
-	const bool qstrand = (A.flag & MM_F_QSTRAND) != 0, filtered = (A.flag & MMB_SKIP_FLAGS) != 0;
+	// heap mode writes reverse hits with the plain formula even in query-strand mode, so the sort below sees the heap merge's keys
+	const bool qstrand = (A.flag & MM_F_QSTRAND) && !(A.flag & MM_F_HEAP_SORT), filtered = (A.flag & MMB_SKIP_FLAGS) != 0;
 	uint32_t w = 0;
 	for (uint32_t j = 0; j < n; ++j) {
 		const uint64_t r = cr[j];
 		bool is_self = false;
 		if (filtered && skip_seed_dev(A, rd, r, q_pos, qlen, &is_self)) continue;
-		const int32_t rpos = (int32_t)((uint32_t)r >> 1);
-		m128 p;
-		if ((r & 1) == (q_pos & 1)) {
-			p.x = (r & 0xffffffff00000000ULL) | (uint32_t)rpos;
-			p.y = (uint64_t)q_span << 32 | q_pos >> 1;
-		} else if (!qstrand) {
-			p.x = 1ULL << 63 | (r & 0xffffffff00000000ULL) | (uint32_t)rpos;
-			p.y = (uint64_t)q_span << 32 | (uint32_t)(qlen - ((int32_t)(q_pos >> 1) + 1 - (int32_t)q_span) - 1);
-		} else {
-			const int32_t len = (int32_t)A.ix.seq_len[r >> 32];
-			p.x = 1ULL << 63 | (r & 0xffffffff00000000ULL) | (uint32_t)(len - (rpos + 1 - (int32_t)q_span) - 1);
-			p.y = (uint64_t)q_span << 32 | q_pos >> 1;
-		}
-		p.y |= (uint64_t)seg_id << MMX_SEED_SEG_SHIFT;
-		if (e >> 31) p.y |= MMX_SEED_TANDEM;
-		if (is_self) p.y |= MMX_SEED_SELF;
-		a[w++] = p;
+		a[w++] = make_anchor(A, r, q, e, is_self, qlen, qstrand);
 	}
 }
 
@@ -420,7 +431,7 @@ __global__ void sort_classify_kernel(const int64_t *a_off, int n_reads, int *cls
 }
 
 __global__ void sort_block_kernel(const m128 *a_in, m128 *a_out, const int64_t *a_off, const int *list, const int *cnt_ptr, int cap,
-								  int *exact_cnt, int *exact_list)
+								  int *exact_cnt, int *exact_list, int tie_min_n)
 {
 	extern __shared__ __align__(16) uint8_t sm_raw[];
 	uint64_t *key = (uint64_t*)sm_raw;
@@ -460,7 +471,7 @@ __global__ void sort_block_kernel(const m128 *a_in, m128 *a_out, const int64_t *
 		}
 		if (tie) s_tie = 1;
 		__syncthreads();
-		if (threadIdx.x == 0 && s_tie && n > 64) exact_list[atomicAdd(exact_cnt, 1)] = rd;
+		if (threadIdx.x == 0 && s_tie && n > tie_min_n) exact_list[atomicAdd(exact_cnt, 1)] = rd;
 		__syncthreads();
 	}
 }
@@ -477,7 +488,7 @@ __global__ void sort_block_kernel(const m128 *a_in, m128 *a_out, const int64_t *
 // reference's unstable radix sort, as before.
 template<int CAP, int NT>
 __global__ void __launch_bounds__(NT, NT >= 1024? 1 : 1024 / NT) sort_radix_kernel(const m128 *a_in, m128 *a_out, const int64_t *a_off, const int *list, const int *cnt_ptr,
-														int *exact_cnt, int *exact_list, int *fallback_cnt, int *fallback_list)
+														int *exact_cnt, int *exact_list, int *fallback_cnt, int *fallback_list, int tie_min_n)
 {
 	constexpr int NW = NT / 32, ITER = CAP / NT, SEG = ITER * 32, RS = NW + 1, NH = 256 * RS, EPT = (NH + NT - 1) / NT;
 	extern __shared__ __align__(16) uint8_t sm_raw[];
@@ -599,7 +610,7 @@ __global__ void __launch_bounds__(NT, NT >= 1024? 1 : 1024 / NT) sort_radix_kern
 		}
 		if (tie) s_tie = 1;
 		__syncthreads();
-		if (tid == 0 && s_tie && n > 64) exact_list[atomicAdd(exact_cnt, 1)] = rd;
+		if (tid == 0 && s_tie && n > tie_min_n) exact_list[atomicAdd(exact_cnt, 1)] = rd;
 		__syncthreads();
 	}
 }
@@ -769,6 +780,70 @@ __global__ void __launch_bounds__(32) sort_exact_smem_kernel(const m128 *a_in, m
 }
 
 
+// ---------------------------------------------------------------------------------------------------------
+// Heap-ordered anchors (collect_seed_hits_heap, map.c:102-166; MM_F_HEAP_SORT). The reference merges the kept seeds' occurrence lists
+// with a min-heap on the occurrence word r and writes forward hits in pop order, then reverse hits in pop order. Occurrence lists are
+// ascending, so pops come in ascending r and both blocks are ascending in x: for a read whose anchors have distinct x this is the
+// stable sort's order. Only the order of equal x depends on the heap's history (equal keys keep sifting down), so the reads with equal
+// adjacent keys after the sort, and the oversize reads the sort kernels do not handle, are replayed here step by step.
+// ---------------------------------------------------------------------------------------------------------
+#define HEAP_SMEM 128 // heap entries per thread in shared memory; reads with more kept seeds keep their heap in global scratch
+
+// ks_heapdown (ksort.h:44-56) with heap_lt(a, b) = a.x > b.x (map.c:74): the smaller child is taken, and the sift stops only below a
+// strictly larger key -- equal keys keep sifting down
+__device__ __forceinline__ void heap_sift_x(m128 *h, int i, int n)
+{
+	const m128 tmp = h[i];
+	int k = i;
+	while ((k = (k << 1) + 1) < n) {
+		if (k != n - 1 && h[k].x > h[k + 1].x) ++k;
+		if (h[k].x > tmp.x) break;
+		h[i] = h[k]; i = k;
+	}
+	h[i] = tmp;
+}
+
+// The replay of one read into a_sorted; h holds n_keep entries {x = r, y = seed << 32 | occurrence}. Every occurrence takes its turn
+// in the heap, also those skip_seed drops.
+__device__ void heap_merge_read(const SeedArgs &A, int rd, m128 *h)
+{
+	const int64_t base = A.mz_off[rd], n = A.a_off[rd + 1] - A.a_off[rd];
+	const int nk = A.n_keep[rd], qlen = A.qlen[rd];
+	const uint32_t *kidx = A.k_idx + base;
+	m128 *out = A.a_sorted + A.a_off[rd];
+	const bool filtered = (A.flag & MMB_SKIP_FLAGS) != 0;
+	for (int i = 0; i < nk; ++i) h[i].x = A.ix.pos[A.s_off[base + (kidx[i] & 0x7fffffffu)]], h[i].y = (uint64_t)i << 32;
+	for (int i = (nk >> 1) - 1; i >= 0; --i) heap_sift_x(h, i, nk); // ks_heapmake
+	int64_t n_for = 0, n_rev = 0;
+	for (int hs = nk; hs > 0;) {
+		const uint64_t r = h[0].x;
+		const uint32_t e = kidx[h[0].y >> 32], mi = e & 0x7fffffffu, j = (uint32_t)h[0].y;
+		const m128 q = A.mz[base + mi];
+		bool is_self = false;
+		if (!(filtered && skip_seed_dev(A, rd, r, (uint32_t)q.y, qlen, &is_self))) {
+			const m128 p = make_anchor(A, r, q, e, is_self, qlen, false);
+			if ((r & 1) == (q.y & 1)) out[n_for++] = p;
+			else out[n - 1 - n_rev++] = p; // reverse hits from the back, in descending pop order
+		}
+		if (j + 1 < A.s_n[base + mi]) h[0].y += 1, h[0].x = A.ix.pos[A.s_off[base + mi] + j + 1];
+		else h[0] = h[--hs];
+		heap_sift_x(h, 0, hs);
+	}
+	for (int64_t k = 0; k < n_rev >> 1; ++k) { const m128 t = out[n_for + k]; out[n_for + k] = out[n - 1 - k]; out[n - 1 - k] = t; }
+}
+
+// One thread per read over two lists (the reads with equal keys, then the oversize reads); scratch: 16 B per minimizer of the batch
+__global__ void __launch_bounds__(32) heap_merge_kernel(SeedArgs A, const int *list0, const int *cnt0, const int *list1, const int *cnt1, m128 *scratch)
+{
+	extern __shared__ __align__(16) uint8_t sm_raw[];
+	m128 *mine = (m128*)sm_raw + (size_t)threadIdx.x * HEAP_SMEM;
+	const int n0 = *cnt0, n_all = n0 + *cnt1;
+	for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_all; t += gridDim.x * blockDim.x) {
+		const int rd = t < n0? list0[t] : list1[t - n0];
+		heap_merge_read(A, rd, A.n_keep[rd] <= HEAP_SMEM? mine : scratch + A.mz_off[rd]);
+	}
+}
+
 } // namespace
 
 // Runs mz-filter, lookup and selection; leaves A.n_a[] filled. Then the caller scans n_a into a_off, sizes the anchor
@@ -778,10 +853,6 @@ void mmb_seed_select_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz)
 	if (A.n_reads <= 0) return;
 	const int rb = (A.n_reads + 127) / 128;
 	ProfScope prof(ctx, MMB_PROF_SEED, (uint64_t)total_mz);
-	if (A.flag & MM_F_HEAP_SORT) {
-		fprintf(stderr, "[ERROR] minimap2_b200: heap-sort seeding (-x sr) is not supported by this build\n");
-		abort();
-	}
 	{
 		const size_t smem = (size_t)MZFLT_SLOTS * 12 + 129 * 4 + 16;
 		static std::once_flag once;
@@ -823,9 +894,14 @@ void mmb_seed_expand_sort_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz, 
 	// sort_exact_kernel's stacks, after the class counters and lists: 16 counters, then (N_CLS+3) lists of n_reads entries: classes,
 	// oversize (index N_CLS), ties (N_CLS+1), fallback of the radix kernels (N_CLS+2)
 	const int N_CLS = 5, CAP0 = 1024; // shared-memory classes: 1024, 2048, 4096, 8192, 16384 anchors
-	int64_t *d_stk_off = mmb_sort_stacks_async(ctx, A.a_off, A.n_reads, total_a, stkbuf, ((size_t)A.n_reads * 8 + 64) * sizeof(int));
+	// heap mode (MM_F_HEAP_SORT): the sort kernels list every read with equal keys, whatever its size, and those reads and the oversize
+	// ones go to heap_merge_kernel instead of the exact emulation; its global-memory heaps (16 B per minimizer) follow the lists
+	const bool heap = (A.flag & MM_F_HEAP_SORT) != 0;
+	const size_t lists_bytes = ((size_t)A.n_reads * 8 + 64) * sizeof(int), heap_bytes = heap? (size_t)total_mz * sizeof(m128) + 16 : 0;
+	int64_t *d_stk_off = mmb_sort_stacks_async(ctx, A.a_off, A.n_reads, total_a, stkbuf, lists_bytes + heap_bytes);
 	int32_t *d_stk = mmb_sort_stacks(d_stk_off, A.n_reads);
 	int *d_cls_cnt = (int*)stkbuf.p, *d_cls_list = d_cls_cnt + 16;
+	const int tie_min_n = heap? 0 : 64; // the radix sort is the reference's order for n <= 64 (insertion sort), the heap merge's is not
 	{
 		ProfScope prof(ctx, MMB_PROF_SORT, (uint64_t)total_a);
 		MMB_CUDA_CHECK(cudaMemsetAsync(d_cls_cnt, 0, 16 * sizeof(int), ctx->stream));
@@ -839,7 +915,7 @@ void mmb_seed_expand_sort_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz, 
 			int per_sm_ = 1; \
 			MMB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_, sort_radix_kernel<CAP_, NT_>, NT_, smem_)); \
 			sort_radix_kernel<CAP_, NT_><<<ctx->n_sm * (per_sm_ > 0? per_sm_ : 1), NT_, smem_, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_cls_list + (size_t)(c_) * A.n_reads, \
-				d_cls_cnt + (c_), d_tie_cnt, d_tie_list, d_fb_cnt, d_fb_list); \
+				d_cls_cnt + (c_), d_tie_cnt, d_tie_list, d_fb_cnt, d_fb_list, tie_min_n); \
 			++ctx->n_launch; } while (0)
 		MMB_RADIX_LAUNCH(1024, 128, 0);
 		MMB_RADIX_LAUNCH(2048, 256, 1);
@@ -854,21 +930,28 @@ void mmb_seed_expand_sort_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz, 
 			int per_sm = 1;
 			MMB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sort_block_kernel, threads, smem));
 			const int grid = ctx->n_sm * (per_sm > 0? per_sm : 1);
-			sort_block_kernel<<<grid, threads, smem, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_fb_list, d_fb_cnt, cap, d_tie_cnt, d_tie_list);
+			sort_block_kernel<<<grid, threads, smem, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_fb_list, d_fb_cnt, cap, d_tie_cnt, d_tie_list, tie_min_n);
+			++ctx->n_launch;
+		}
+		if (heap) { // heap merge replay of the reads with equal keys and of the oversize reads
+			const size_t smem = (size_t)32 * HEAP_SMEM * sizeof(m128);
+			{ static std::once_flag once; std::call_once(once, [&]() { MMB_CUDA_CHECK(cudaFuncSetAttribute(heap_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); }); }
+			m128 *scratch = (m128*)(((uintptr_t)stkbuf.p + lists_bytes + 15) & ~(uintptr_t)15);
+			heap_merge_kernel<<<ctx->n_sm * 3, 32, smem, ctx->stream>>>(A, d_tie_list, d_tie_cnt, d_cls_list + (size_t)N_CLS * A.n_reads, d_cls_cnt + N_CLS, scratch);
 			++ctx->n_launch;
 		}
 		// exact emulation: reads with equal keys go through the shared-memory walker (cap 15360 anchors: 12 B/entry + per-lane bucket tables);
 		// whatever does not fit, and the oversize class, falls back to the global-memory walker (one thread per read)
-		{
+		else {
 			const int cap = 15360;
 			const size_t smem = (size_t)cap * 12 + 32 * 512 * 2 + 2 * 512 * 4;
 			{ static std::once_flag once; std::call_once(once, [&]() { MMB_CUDA_CHECK(cudaFuncSetAttribute(sort_exact_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->smem_optin - 1024)); }); }
 			sort_exact_smem_kernel<<<ctx->n_sm, 32, smem, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_cls_list + (size_t)(N_CLS + 1) * A.n_reads, d_cls_cnt + N_CLS + 1,
 																		 cap, d_cls_cnt + N_CLS, d_cls_list + (size_t)N_CLS * A.n_reads);
 			++ctx->n_launch;
+			sort_exact_kernel<<<(A.n_reads + 63) / 64, 64, 0, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_cls_list + (size_t)N_CLS * A.n_reads, d_cls_cnt + N_CLS, d_stk, d_stk_off);
+			++ctx->n_launch;
 		}
-		sort_exact_kernel<<<(A.n_reads + 63) / 64, 64, 0, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_cls_list + (size_t)N_CLS * A.n_reads, d_cls_cnt + N_CLS, d_stk, d_stk_off);
-		++ctx->n_launch;
 		static const bool dbg = getenv("MM_B200_SORT_STATS") != nullptr;
 		if (dbg) { // development aid: reads per class / oversize / with equal keys / fallback
 			int h[16];
