@@ -254,6 +254,20 @@ int64_t mmb_seed_batch_host(mmb_ctx_t *ctx, const mm_idx_t *mi, int n_reads, con
 							float q_occ_frac, int max_max_occ, int occ_dist, int64_t *a_off_out, int32_t *rep_len_out, int32_t *n_mini_out,
 							uint64_t *anchors_xy, int64_t a_cap, uint64_t *mini_pos, int64_t mp_cap);
 
+/* The anchor sort of the seeding stage alone (radix_sort_128x, map.c:202), for kernel-level tests: the anchors of each read
+ * (anchors_xy[a_off[i], a_off[i+1]), 16 B each) are sorted by x into sorted_xy as the stage does without MM_F_HEAP_SORT, equal keys in
+ * the reference's order. route (if non-null) receives one code per read: the size class (0-4: radix sort in shared memory for at most
+ * 1024 << class anchors; MMB_SORT_ROUTE_OVERSIZE: more than 16384), plus MMB_SORT_ROUTE_NETWORK when the keys vary in more than 33
+ * bits (network sort), MMB_SORT_ROUTE_EXACT when the read was listed for the exact emulation of the unstable sort (equal keys and more
+ * than 64 anchors), MMB_SORT_ROUTE_GLOBAL when the shared-memory exact walker passed it on to the global-memory one; a read without
+ * anchors gets MMB_SORT_ROUTE_NONE. Returns the total number of anchors. */
+#define MMB_SORT_ROUTE_NONE (-1)
+#define MMB_SORT_ROUTE_OVERSIZE 5
+#define MMB_SORT_ROUTE_NETWORK 8
+#define MMB_SORT_ROUTE_EXACT 16
+#define MMB_SORT_ROUTE_GLOBAL 32
+int64_t mmb_anchor_sort_host(mmb_ctx_t *ctx, int n_reads, const uint64_t *anchors_xy, const int64_t *a_off, uint64_t *sorted_xy, int32_t *route);
+
 /* synthetic workload for bench.py (BASELINE.json configs[1] shape; there is no network for real genomes): a random
  * genome of total_len bases in n_contigs contigs indexed on the device, and reads sampled from it with the given
  * error profile (err = per-base error rate, split into substitutions / insertions / deletions by sub, ins, 1-sub-ins). */

@@ -75,8 +75,16 @@ def lib():
                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.mmb_idx_lookup_host.restype = C.c_int64
         L.mmb_idx_lookup_host.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
+        declare_anchor_sort(L)
         _lib = L
     return _lib
+
+
+def declare_anchor_sort(L):
+    """argtypes of mmb_anchor_sort_host on L (this package's library, or a build of the same sources)"""
+    L.mmb_anchor_sort_host.restype = C.c_int64
+    L.mmb_anchor_sort_host.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    return L
 
 
 class Context:

@@ -31,6 +31,22 @@ struct SeedArgs {
 void mmb_seed_select_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz);
 void mmb_seed_expand_sort_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz, int64_t total_a, DevBuf &stkbuf);
 
+// The anchor sort (radix_sort_128x, map.c:202) of n_reads reads: a_in[a_off[i], a_off[i+1]) sorted by x into a_out at the same offsets.
+// Each read goes by its anchor count to one of the shared-memory radix classes or to the oversize list. The radix kernels hand reads
+// whose keys vary in more than 33 bits to the network sort, and list the reads with equal keys and more than tie_min_n anchors. With
+// run_exact, the listed reads and the oversize ones are then re-sorted by the exact emulation of the reference's unstable sort; without
+// it the caller orders them (heap mode). The returned counters and lists live in stkbuf, in device memory: cnt[c] reads in
+// list + c * n_reads, for c = 0..4 (radix class of at most 1024 << c anchors), MMB_SORT_OVERSIZE (more than 16384 anchors, and the
+// listed reads the shared-memory exact walker passes on), MMB_SORT_TIES and MMB_SORT_FALLBACK (network sort). extra: extra_bytes of
+// 16-byte aligned device scratch for the caller, after the lists.
+enum { MMB_SORT_N_CLS = 5, MMB_SORT_OVERSIZE = 5, MMB_SORT_TIES = 6, MMB_SORT_FALLBACK = 7 };
+// tie_min_n of the sorted order: the reference sorts up to 64 anchors by a stable insertion sort (ksort.h:147), so only larger reads with
+// equal keys need the exact emulation
+enum { MMB_SORT_TIE_MIN_N = 64 };
+struct AnchorSortLists { int *cnt, *list; void *extra; };
+AnchorSortLists mmb_anchor_sort_device(mmb_ctx_t *ctx, const m128 *a_in, m128 *a_out, const int64_t *d_a_off, int n_reads, int64_t total_a,
+										int tie_min_n, bool run_exact, DevBuf &stkbuf, size_t extra_bytes);
+
 void mmb_chain_device(mmb_ctx_t *ctx, const mmb_chain_par_t *par, int n_reads, const m128 *d_a, const int64_t *d_a_off, int64_t n_tot,
 					  int32_t *d_n_u, int32_t *d_n_v, uint64_t *d_u, m128 *d_a_out, DevBuf &scratch, DevBuf &scratch2);
 

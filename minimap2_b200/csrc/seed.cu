@@ -881,40 +881,29 @@ void mmb_seed_select_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz)
 	MMB_CUDA_CHECK(cudaGetLastError());
 }
 
-void mmb_seed_expand_sort_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz, int64_t total_a, DevBuf &stkbuf)
+AnchorSortLists mmb_anchor_sort_device(mmb_ctx_t *ctx, const m128 *a_in, m128 *a_out, const int64_t *d_a_off, int n_reads, int64_t total_a,
+										int tie_min_n, bool run_exact, DevBuf &stkbuf, size_t extra_bytes)
 {
-	if (A.n_reads <= 0) return;
-	{
-		ProfScope prof(ctx, MMB_PROF_SEED, 0);
-		if (total_mz > 0) {
-			expand_kernel<<<(unsigned)((total_mz + 255) / 256), 256, 0, ctx->stream>>>(A, total_mz);
-			++ctx->n_launch;
-		}
-	}
 	// sort_exact_kernel's stacks, after the class counters and lists: 16 counters, then (N_CLS+3) lists of n_reads entries: classes,
-	// oversize (index N_CLS), ties (N_CLS+1), fallback of the radix kernels (N_CLS+2)
-	const int N_CLS = 5, CAP0 = 1024; // shared-memory classes: 1024, 2048, 4096, 8192, 16384 anchors
-	// heap mode (MM_F_HEAP_SORT): the sort kernels list every read with equal keys, whatever its size, and those reads and the oversize
-	// ones go to heap_merge_kernel instead of the exact emulation; its global-memory heaps (16 B per minimizer) follow the lists
-	const bool heap = (A.flag & MM_F_HEAP_SORT) != 0;
-	const size_t lists_bytes = ((size_t)A.n_reads * 8 + 64) * sizeof(int), heap_bytes = heap? (size_t)total_mz * sizeof(m128) + 16 : 0;
-	int64_t *d_stk_off = mmb_sort_stacks_async(ctx, A.a_off, A.n_reads, total_a, stkbuf, lists_bytes + heap_bytes);
-	int32_t *d_stk = mmb_sort_stacks(d_stk_off, A.n_reads);
+	// oversize (index N_CLS), ties (N_CLS+1), fallback of the radix kernels (N_CLS+2); then the caller's extra bytes
+	const int N_CLS = MMB_SORT_N_CLS, CAP0 = 1024; // shared-memory classes: 1024, 2048, 4096, 8192, 16384 anchors
+	const size_t lists_bytes = ((size_t)n_reads * 8 + 64) * sizeof(int);
+	int64_t *d_stk_off = mmb_sort_stacks_async(ctx, d_a_off, n_reads, total_a, stkbuf, lists_bytes + extra_bytes);
+	int32_t *d_stk = mmb_sort_stacks(d_stk_off, n_reads);
 	int *d_cls_cnt = (int*)stkbuf.p, *d_cls_list = d_cls_cnt + 16;
-	const int tie_min_n = heap? 0 : 64; // the radix sort is the reference's order for n <= 64 (insertion sort), the heap merge's is not
 	{
 		ProfScope prof(ctx, MMB_PROF_SORT, (uint64_t)total_a);
 		MMB_CUDA_CHECK(cudaMemsetAsync(d_cls_cnt, 0, 16 * sizeof(int), ctx->stream));
-		sort_classify_kernel<<<(A.n_reads + 255) / 256, 256, 0, ctx->stream>>>(A.a_off, A.n_reads, d_cls_cnt, d_cls_list, N_CLS, CAP0);
+		sort_classify_kernel<<<(n_reads + 255) / 256, 256, 0, ctx->stream>>>(d_a_off, n_reads, d_cls_cnt, d_cls_list, N_CLS, CAP0);
 		++ctx->n_launch;
-		int *d_tie_cnt = d_cls_cnt + N_CLS + 1, *d_tie_list = d_cls_list + (size_t)(N_CLS + 1) * A.n_reads;
-		int *d_fb_cnt = d_cls_cnt + N_CLS + 2, *d_fb_list = d_cls_list + (size_t)(N_CLS + 2) * A.n_reads;
+		int *d_tie_cnt = d_cls_cnt + N_CLS + 1, *d_tie_list = d_cls_list + (size_t)(N_CLS + 1) * n_reads;
+		int *d_fb_cnt = d_cls_cnt + N_CLS + 2, *d_fb_list = d_cls_list + (size_t)(N_CLS + 2) * n_reads;
 		#define MMB_RADIX_LAUNCH(CAP_, NT_, c_) do { \
 			const size_t smem_ = (size_t)(CAP_) * 12 + (size_t)256 * ((NT_) / 32 + 1) * 2; \
 			{ static std::once_flag once_; std::call_once(once_, [&]() { MMB_CUDA_CHECK(cudaFuncSetAttribute(sort_radix_kernel<CAP_, NT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_)); }); } \
 			int per_sm_ = 1; \
 			MMB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_, sort_radix_kernel<CAP_, NT_>, NT_, smem_)); \
-			sort_radix_kernel<CAP_, NT_><<<ctx->n_sm * (per_sm_ > 0? per_sm_ : 1), NT_, smem_, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_cls_list + (size_t)(c_) * A.n_reads, \
+			sort_radix_kernel<CAP_, NT_><<<ctx->n_sm * (per_sm_ > 0? per_sm_ : 1), NT_, smem_, ctx->stream>>>(a_in, a_out, d_a_off, d_cls_list + (size_t)(c_) * n_reads, \
 				d_cls_cnt + (c_), d_tie_cnt, d_tie_list, d_fb_cnt, d_fb_list, tie_min_n); \
 			++ctx->n_launch; } while (0)
 		MMB_RADIX_LAUNCH(1024, 128, 0);
@@ -930,35 +919,84 @@ void mmb_seed_expand_sort_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz, 
 			int per_sm = 1;
 			MMB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sort_block_kernel, threads, smem));
 			const int grid = ctx->n_sm * (per_sm > 0? per_sm : 1);
-			sort_block_kernel<<<grid, threads, smem, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_fb_list, d_fb_cnt, cap, d_tie_cnt, d_tie_list, tie_min_n);
-			++ctx->n_launch;
-		}
-		if (heap) { // heap merge replay of the reads with equal keys and of the oversize reads
-			const size_t smem = (size_t)32 * HEAP_SMEM * sizeof(m128);
-			{ static std::once_flag once; std::call_once(once, [&]() { MMB_CUDA_CHECK(cudaFuncSetAttribute(heap_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); }); }
-			m128 *scratch = (m128*)(((uintptr_t)stkbuf.p + lists_bytes + 15) & ~(uintptr_t)15);
-			heap_merge_kernel<<<ctx->n_sm * 3, 32, smem, ctx->stream>>>(A, d_tie_list, d_tie_cnt, d_cls_list + (size_t)N_CLS * A.n_reads, d_cls_cnt + N_CLS, scratch);
+			sort_block_kernel<<<grid, threads, smem, ctx->stream>>>(a_in, a_out, d_a_off, d_fb_list, d_fb_cnt, cap, d_tie_cnt, d_tie_list, tie_min_n);
 			++ctx->n_launch;
 		}
 		// exact emulation: reads with equal keys go through the shared-memory walker (cap 15360 anchors: 12 B/entry + per-lane bucket tables);
 		// whatever does not fit, and the oversize class, falls back to the global-memory walker (one thread per read)
-		else {
+		if (run_exact) {
 			const int cap = 15360;
 			const size_t smem = (size_t)cap * 12 + 32 * 512 * 2 + 2 * 512 * 4;
 			{ static std::once_flag once; std::call_once(once, [&]() { MMB_CUDA_CHECK(cudaFuncSetAttribute(sort_exact_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->smem_optin - 1024)); }); }
-			sort_exact_smem_kernel<<<ctx->n_sm, 32, smem, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_cls_list + (size_t)(N_CLS + 1) * A.n_reads, d_cls_cnt + N_CLS + 1,
-																		 cap, d_cls_cnt + N_CLS, d_cls_list + (size_t)N_CLS * A.n_reads);
+			sort_exact_smem_kernel<<<ctx->n_sm, 32, smem, ctx->stream>>>(a_in, a_out, d_a_off, d_tie_list, d_tie_cnt,
+																		 cap, d_cls_cnt + N_CLS, d_cls_list + (size_t)N_CLS * n_reads);
 			++ctx->n_launch;
-			sort_exact_kernel<<<(A.n_reads + 63) / 64, 64, 0, ctx->stream>>>(A.a, A.a_sorted, A.a_off, d_cls_list + (size_t)N_CLS * A.n_reads, d_cls_cnt + N_CLS, d_stk, d_stk_off);
+			sort_exact_kernel<<<(n_reads + 63) / 64, 64, 0, ctx->stream>>>(a_in, a_out, d_a_off, d_cls_list + (size_t)N_CLS * n_reads, d_cls_cnt + N_CLS, d_stk, d_stk_off);
 			++ctx->n_launch;
-		}
-		static const bool dbg = getenv("MM_B200_SORT_STATS") != nullptr;
-		if (dbg) { // development aid: reads per class / oversize / with equal keys / fallback
-			int h[16];
-			MMB_CUDA_CHECK(cudaMemcpyAsync(h, d_cls_cnt, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
-			MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-			fprintf(stderr, "[sort] reads=%d anchors=%lld classes=%d/%d/%d/%d/%d oversize=%d ties=%d fallback=%d\n", A.n_reads, (long long)total_a, h[0], h[1], h[2], h[3], h[4], h[5], h[6], h[7]);
 		}
 	}
 	MMB_CUDA_CHECK(cudaGetLastError());
+	return AnchorSortLists{d_cls_cnt, d_cls_list, (void*)(((uintptr_t)stkbuf.p + lists_bytes + 15) & ~(uintptr_t)15)};
+}
+
+void mmb_seed_expand_sort_device(mmb_ctx_t *ctx, SeedArgs &A, int64_t total_mz, int64_t total_a, DevBuf &stkbuf)
+{
+	if (A.n_reads <= 0) return;
+	{
+		ProfScope prof(ctx, MMB_PROF_SEED, 0);
+		if (total_mz > 0) {
+			expand_kernel<<<(unsigned)((total_mz + 255) / 256), 256, 0, ctx->stream>>>(A, total_mz);
+			++ctx->n_launch;
+		}
+	}
+	// heap mode (MM_F_HEAP_SORT): the sort kernels list every read with equal keys, whatever its size, and those reads and the oversize
+	// ones go to heap_merge_kernel instead of the exact emulation; its global-memory heaps (16 B per minimizer) follow the lists
+	const bool heap = (A.flag & MM_F_HEAP_SORT) != 0;
+	const size_t heap_bytes = heap? (size_t)total_mz * sizeof(m128) + 16 : 0;
+	const int tie_min_n = heap? 0 : MMB_SORT_TIE_MIN_N; // the radix sort is the reference's order for n <= 64 (insertion sort), the heap merge's is not
+	const AnchorSortLists S = mmb_anchor_sort_device(ctx, A.a, A.a_sorted, A.a_off, A.n_reads, total_a, tie_min_n, !heap, stkbuf, heap_bytes);
+	if (heap) { // heap merge replay of the reads with equal keys and of the oversize reads
+		ProfScope prof(ctx, MMB_PROF_SORT, 0);
+		const size_t smem = (size_t)32 * HEAP_SMEM * sizeof(m128);
+		{ static std::once_flag once; std::call_once(once, [&]() { MMB_CUDA_CHECK(cudaFuncSetAttribute(heap_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); }); }
+		heap_merge_kernel<<<ctx->n_sm * 3, 32, smem, ctx->stream>>>(A, S.list + (size_t)MMB_SORT_TIES * A.n_reads, S.cnt + MMB_SORT_TIES,
+																	 S.list + (size_t)MMB_SORT_OVERSIZE * A.n_reads, S.cnt + MMB_SORT_OVERSIZE, (m128*)S.extra);
+		++ctx->n_launch;
+		MMB_CUDA_CHECK(cudaGetLastError());
+	}
+}
+
+// Kernel-level entry for tests: the anchor sort alone on caller-given anchors, as the seeding stage runs it without MM_F_HEAP_SORT.
+// route (if non-null) receives each read's path, read back from the class counters and lists (MMB_SORT_ROUTE_*, include/mm_b200.h).
+extern "C" int64_t mmb_anchor_sort_host(mmb_ctx_t *ctx, int n_reads, const uint64_t *anchors_xy, const int64_t *a_off, uint64_t *sorted_xy, int32_t *route)
+{
+	if (n_reads <= 0) return 0;
+	MMB_CUDA_CHECK(cudaSetDevice(ctx->device));
+	const int64_t n_tot = a_off[n_reads];
+	m128 *d_in = ctx->d_a.as<m128>((size_t)n_tot + 1), *d_out = ctx->d_b.as<m128>((size_t)n_tot + 1);
+	int64_t *d_off = ctx->d_c.as<int64_t>((size_t)n_reads + 1);
+	MMB_CUDA_CHECK(cudaMemcpyAsync(d_in, anchors_xy, sizeof(m128) * n_tot, cudaMemcpyHostToDevice, ctx->stream));
+	MMB_CUDA_CHECK(cudaMemcpyAsync(d_off, a_off, sizeof(int64_t) * (n_reads + 1), cudaMemcpyHostToDevice, ctx->stream));
+	const AnchorSortLists S = mmb_anchor_sort_device(ctx, d_in, d_out, d_off, n_reads, n_tot, MMB_SORT_TIE_MIN_N, true, ctx->d_d, 0);
+	MMB_CUDA_CHECK(cudaMemcpyAsync(sorted_xy, d_out, sizeof(m128) * n_tot, cudaMemcpyDeviceToHost, ctx->stream));
+	if (route) {
+		const int n_lists = MMB_SORT_FALLBACK + 1;
+		int cnt[n_lists];
+		std::vector<int> lists((size_t)n_lists * n_reads);
+		MMB_CUDA_CHECK(cudaMemcpyAsync(cnt, S.cnt, sizeof(cnt), cudaMemcpyDeviceToHost, ctx->stream));
+		MMB_CUDA_CHECK(cudaMemcpyAsync(lists.data(), S.list, sizeof(int) * lists.size(), cudaMemcpyDeviceToHost, ctx->stream));
+		MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+		for (int i = 0; i < n_reads; ++i) route[i] = MMB_SORT_ROUTE_NONE;
+		for (int c = 0; c < n_lists; ++c) { // the size classes first: the oversize list also holds the reads the shared-memory exact walker passed on
+			const int *l = lists.data() + (size_t)c * n_reads;
+			for (int j = 0; j < cnt[c]; ++j) {
+				int32_t &r = route[l[j]];
+				if (c < MMB_SORT_N_CLS) r = c;
+				else if (c == MMB_SORT_OVERSIZE) r = r == MMB_SORT_ROUTE_NONE? MMB_SORT_ROUTE_OVERSIZE : r | MMB_SORT_ROUTE_GLOBAL;
+				else r |= c == MMB_SORT_TIES? MMB_SORT_ROUTE_EXACT : MMB_SORT_ROUTE_NETWORK;
+			}
+		}
+	}
+	MMB_CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+	return n_tot;
 }

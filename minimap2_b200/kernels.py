@@ -129,6 +129,26 @@ def idx_lookup(idx, keys, L=None):
     return cnt[:n], occ_off, occ[:tot]
 
 
+SORT_ROUTE_NONE, SORT_ROUTE_OVERSIZE, SORT_ROUTE_NETWORK, SORT_ROUTE_EXACT, SORT_ROUTE_GLOBAL = -1, 5, 8, 16, 32  # MMB_SORT_ROUTE_*
+
+
+def anchor_sort_batch(ctx, arrays, L=None):
+    """The seeding stage's anchor sort (radix_sort_128x) on every read. arrays: list of (n_i, 2) uint64 anchor arrays. Returns (sorted
+    arrays, routes): routes[i] is read i's path through the sort kernels (MMB_SORT_ROUTE_* in include/mm_b200.h). ctx: a Context or a
+    context handle; L: the library to call (default: this package's; declare_anchor_sort() gives another one the argtypes)."""
+    n = len(arrays)
+    off = np.zeros(n + 1, dtype=np.int64)
+    for i, a in enumerate(arrays):
+        off[i + 1] = off[i] + len(a)
+    tot = int(off[-1])
+    cat = np.ascontiguousarray(np.concatenate([np.asarray(a, dtype=np.uint64).reshape(-1, 2) for a in arrays]) if tot else np.zeros((1, 2), dtype=np.uint64))
+    out = np.zeros((max(tot, 1), 2), dtype=np.uint64)
+    route = np.zeros(max(n, 1), dtype=np.int32)
+    got = (L or lib()).mmb_anchor_sort_host(getattr(ctx, "h", ctx), n, cat.ctypes.data, off.ctypes.data, out.ctypes.data, route.ctypes.data)
+    assert got == tot, (got, tot)
+    return [out[int(off[i]):int(off[i + 1])].copy() for i in range(n)], route[:n]
+
+
 class JumpHit(C.Structure):  # mmb_jump_hit_t (include/mm_b200.h)
     _fields_ = [("rid", C.c_int32), ("rs", C.c_int32), ("re", C.c_int32), ("qs", C.c_int32), ("qe", C.c_int32), ("rev", C.c_int32),
                 ("qlen", C.c_int32), ("n_cigar", C.c_int32), ("q_off", C.c_int64), ("cig_first", C.c_uint32), ("cig_last", C.c_uint32)]

@@ -9,7 +9,6 @@ import argparse
 import ctypes as C
 import json
 import os
-import re
 import subprocess
 import sys
 import time
@@ -32,27 +31,43 @@ def workloads(L, idx, a):
     return out
 
 
+def reads_with_ties(L, idx, opt, flag, buf, qlens, chunk=2000):
+    """reads whose sorted anchors (first seeding pass, at mid_occ) have equal neighbouring keys and at most 16384 anchors: the reads the
+    sort kernels list for the heap merge in heap mode"""
+    L.mmb_seed_batch_host.restype = C.c_int64
+    L.mmb_seed_batch_host.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_float, C.c_int, C.c_int,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]
+    ctx = L.mmb_ctx_create(0)
+    off_all = np.concatenate([[0], np.cumsum(qlens, dtype=np.int64)])
+    n_tie = 0
+    for r0 in range(0, len(qlens), chunk):
+        r1 = min(r0 + chunk, len(qlens))
+        off = off_all[r0:r1 + 1] - off_all[r0]
+        seq = np.concatenate([buf[off_all[r0]:off_all[r1]], np.zeros(1, dtype=np.uint8)])
+        a_off = np.zeros(r1 - r0 + 1, dtype=np.int64); rep = np.zeros(r1 - r0, dtype=np.int32); nmini = np.zeros(r1 - r0, dtype=np.int32)
+        a = np.zeros((1, 2), dtype=np.uint64)
+        for _ in range(2):  # the second call with room for every anchor
+            tot = L.mmb_seed_batch_host(ctx, idx, r1 - r0, seq.ctypes.data, off.ctypes.data, flag, opt.mid_occ, opt.q_occ_frac, opt.max_max_occ,
+                                        opt.occ_dist, a_off.ctypes.data, rep.ctypes.data, nmini.ctypes.data, a.ctypes.data, len(a), None, 0)
+            if tot >= 0:
+                break
+            a = np.zeros((int(a_off[-1]) + 1, 2), dtype=np.uint64)
+        eq = np.zeros(len(a), dtype=bool)
+        eq[1:] = a[1:, 0] == a[:-1, 0]
+        for i in range(r1 - r0):
+            s, e = int(a_off[i]), int(a_off[i + 1])
+            n_tie += int(e - s <= 16384 and eq[s + 1:e].any())
+    L.mmb_ctx_destroy(ctx)
+    return n_tie
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--genome-mbp", type=float, default=3000.0)
     ap.add_argument("--long-reads", type=int, default=30000)
     ap.add_argument("--short-reads", type=int, default=1_000_000)
     ap.add_argument("--rounds", type=int, default=2)
-    ap.add_argument("--count-ties", action="store_true", help=argparse.SUPPRESS)
     a = ap.parse_args()
-    ties = {}
-    if not a.count_ties:  # first, while this process holds no device memory: the child maps once in heap mode with the sort statistics on
-        p = subprocess.run([sys.executable, os.path.abspath(__file__), "--count-ties", "--genome-mbp", str(a.genome_mbp), "--long-reads", str(a.long_reads),
-                            "--short-reads", str(a.short_reads)], env=dict(os.environ, MM_B200_SORT_STATS="1"), stdout=subprocess.PIPE, stderr=subprocess.PIPE)
-        assert p.returncode == 0, p.stderr.decode()[-2000:]
-        cur = None
-        for l in p.stderr.decode().splitlines():
-            if l.startswith("[workload] "):
-                cur = l.split()[1]
-                ties[cur] = 0
-            m = re.search(r" ties=(\d+)", l)
-            if m and cur:
-                ties[cur] += int(m.group(1))
     L = api._setup()
     L.mmb_profile_ms_all.restype = C.c_double
     L.mmb_launch_count_all.restype = C.c_uint64
@@ -60,13 +75,6 @@ def main():
     al = Aligner(preset="map-ont", _idx=idx, n_threads=16)
     base_flag = al.map_opt.flag
     wls = workloads(L, idx, a)
-    if a.count_ties:  # child: one heap-mode mapping per workload, the sort statistics go to stderr
-        al.map_opt.flag = base_flag | HEAP
-        for tag, buf, qlens in wls:
-            print("[workload] " + tag, file=sys.stderr, flush=True)
-            nr, rg, _ = al.map_prepared(al.prepare_batch(buf, qlens))
-            Aligner.free_batch(nr, rg)
-        return
     res = {}
     for tag, buf, qlens in wls:
         prep = al.prepare_batch(buf, qlens)
@@ -97,7 +105,7 @@ def main():
             L.mmb_profile_enable_all(0)
             L.mmb_set_groups(0)
             r[m]["map_s"] = round(min(r[m]["map_s"]), 4)
-        res[tag] = dict(n_reads=len(qlens), read_len=int(qlens[0]), reads_with_ties=ties[tag], **{"heap_" + m: v for m, v in r.items()})
+        res[tag] = dict(n_reads=len(qlens), read_len=int(qlens[0]), reads_with_ties=reads_with_ties(L, idx, al.map_opt, base_flag, buf, qlens), **{"heap_" + m: v for m, v in r.items()})
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], stdout=subprocess.PIPE).stdout.decode().strip()
     print(json.dumps(dict(gpu=gpu, genome_mbp=a.genome_mbp, workloads=res)))
 

@@ -82,3 +82,121 @@ def repeat_rich_case(seed, glen, n_reads, rlen, rep=0.4, n_contigs=2):
     reads.append(bytes(contigs[0][500:900]) * 5)
     reads.append(b"ACGT")
     return contigs, reads
+
+
+def n_sketch(seq, w, k):
+    """minimizers of a read before the query-side filter"""
+    return len(O.oracle_sketch(bytes(seq), w, k))
+
+
+def trim_to_count(seq, target, count):
+    """the shortest prefix of seq with count(prefix) == target minimizers (count: n_sketch or n_minimizers with their parameters bound)"""
+    lo, hi = 0, len(seq)
+    assert count(seq) >= target, (count(seq), target)
+    while lo < hi:  # the shortest prefix with at least target
+        mid = (lo + hi) // 2
+        if count(seq[:mid]) >= target:
+            hi = mid
+        else:
+            lo = mid + 1
+    for ln in range(lo, min(len(seq), lo + 64) + 1):
+        if count(seq[:ln]) == target:
+            return bytes(seq[:ln])
+    raise ValueError("no prefix with %d minimizers" % target)
+
+
+def read_counts(seq, w, k):
+    """how often each minimizer of the read occurs in it (what mm_seed_mz_flt compares with q_occ_max and n * q_occ_frac)"""
+    _, cnt = np.unique(O.oracle_sketch(bytes(seq), w, k)[:, 0], return_counts=True)
+    return cnt
+
+
+def streaks(seq, contigs, w, k, max_occ, occ_dist):
+    """mm_seed_select's stretches of seeds with more than max_occ occurrences (seed.c:56-96), from the oracle's sketches: per stretch,
+    (its number of seeds, max_high_occ = (pe - ps) / occ_dist + .499) before the 128-entry cap"""
+    occ = {}
+    for c in contigs:
+        for x in O.oracle_sketch(bytes(c), w, k)[:, 0] >> np.uint64(8):
+            occ[int(x)] = occ.get(int(x), 0) + 1
+    mz = O.oracle_sketch(bytes(seq), w, k)
+    seeds = [(int(y & np.uint64(0xffffffff)) >> 1, occ[int(x >> np.uint64(8))]) for x, y in mz if int(x >> np.uint64(8)) in occ]
+    out, last0 = [], -1
+    for i in range(len(seeds) + 1):
+        if i == len(seeds) or seeds[i][1] <= max_occ:
+            if i - last0 > 1:
+                ps = 0 if last0 < 0 else seeds[last0][0]
+                pe = len(seq) if i == len(seeds) else seeds[i][0]
+                out.append((i - last0 - 1, int((pe - ps) / occ_dist + .499)))
+            last0 = i
+    return out
+
+
+def edge_genome(seed):
+    """a random genome with a 2 kb segment copied 20 times (seeds with 20 occurrences: high-occurrence stretches) and tandem arrays of a
+    40-bp, a 37-bp and a 7-bp unit (minimizers that occur many times in one read)"""
+    rng = np.random.default_rng(seed)
+    rnd = lambda n: bytes(synth.ALPHA[rng.integers(0, 4, n)])
+    rep, u40, u37, u7 = rnd(2000), rnd(40), rnd(37), b"ACGGTCA"
+    ctg0 = b"".join(rnd(3000) + rep for _ in range(20)) + rnd(3000)
+    ctg1 = rnd(20_000) + u40 * 40 + rnd(500) + u37 * 11 + rnd(500) + u7 * 12 + rnd(20_000)
+    return [ctg0, ctg1], dict(rep=rep, u40=u40, u37=u37, u7=u7, flank=ctg1[:20_000], rnd=rnd)
+
+
+def mzflt_edge_reads(parts, w=10, k=15, q_occ_max=10):
+    """reads of exactly 2048 and 2049 minimizers before the query-side filter (mzflt_smem_kernel / mzflt_kernel), each opening with
+    tandem arrays whose minimizers occur q_occ_max times and more in the read; reads of q_occ_max and q_occ_max + 1 minimizers of one
+    7-bp unit (the filter's n <= q_occ_max exit)"""
+    body = parts["u37"] * 11 + parts["u40"] * 40 + parts["flank"] + parts["rnd"](20_000)
+    out = [trim_to_count(body, n, lambda s: n_sketch(s, w, k)) for n in (2048, 2049)]
+    out += [trim_to_count(parts["u7"] * 40, n, lambda s: n_sketch(s, w, k)) for n in (q_occ_max, q_occ_max + 1)]
+    return out
+
+
+def select_edge_reads(parts, w=10, k=15):
+    """reads of exactly 2048 and 2049 minimizers (SEL_CAP: select_kernel's shared or global seed tables) that open with copies of the
+    repeated segment, so streak selection has stretches of high-occurrence seeds to thin"""
+    body = parts["rep"] + parts["flank"] + parts["rep"][:900] + parts["rnd"](20_000)
+    return [trim_to_count(body, n, lambda s: n_sketch(s, w, k)) for n in (2048, 2049)]
+
+
+def streak_edge_reads(contigs, parts, w=10, k=15, max_occ=10, occ_dist=10, want=(128, 129)):
+    """one stretch of high-occurrence seeds (a prefix of the repeated segment between unique flanks) per wanted max_high_occ; the stretch
+    length is searched with streaks()"""
+    fl0, fl1 = parts["flank"][:300], parts["flank"][5000:5300]
+    found = {}
+    for ln in range(1100, 1500):
+        s = fl0 + parts["rep"][:ln] + fl1
+        st = streaks(s, contigs, w, k, max_occ, occ_dist)
+        for n_seed, mho in st:
+            if mho in want and mho not in found and n_seed > mho:
+                found[mho] = s
+        if len(found) == len(want):
+            break
+    assert len(found) == len(want), sorted(found)
+    return [found[m] for m in want] + [fl0 + parts["rep"] + fl1]
+
+
+def check_edges(L, ctx, seed=3, w=10, k=15, q_occ_max=10):
+    """the seeding stage at its capacity edges against the oracle, each case first asserting from the oracle side that both sides of its
+    boundary occur: 2048 / 2049 minimizers before the query-side filter with entries both filter kernels drop (one occurring exactly
+    q_occ_max times); q_occ_max / q_occ_max + 1 minimizers; 2048 / 2049 minimizers in select_kernel with streak selection on; stretches
+    whose max_high_occ is 128, 129 and far above the streak heap's 128 entries"""
+    contigs, parts = edge_genome(seed)
+    mz = mzflt_edge_reads(parts, w, k, q_occ_max)
+    frac = 0.001  # n * q_occ_frac < q_occ_max: q_occ_max decides
+    assert [n_sketch(s, w, k) for s in mz] == [2048, 2049, q_occ_max, q_occ_max + 1]
+    for s in mz[:2]:
+        cnt = read_counts(s, w, k)
+        assert (cnt == q_occ_max).any() and (cnt > q_occ_max).any() and q_occ_max > n_sketch(s, w, k) * frac
+        assert n_minimizers(s, w, k, q_occ_max, frac) < n_sketch(s, w, k)
+    assert n_minimizers(mz[2], w, k, q_occ_max, frac) == q_occ_max and n_minimizers(mz[3], w, k, q_occ_max, frac) == 0
+    check_case(L, ctx, contigs, mz, w=w, k=k, mid_occ=q_occ_max, q_occ_frac=frac)
+    sel = select_edge_reads(parts, w, k)
+    assert [n_sketch(s, w, k) for s in sel] == [2048, 2049]
+    for s in sel:
+        assert any(n_seed > mho > 0 for n_seed, mho in streaks(s, contigs, w, k, q_occ_max, 200))
+    check_case(L, ctx, contigs, sel, w=w, k=k, mid_occ=q_occ_max, q_occ_frac=0.0, occ_dist=200)
+    stk = streak_edge_reads(contigs, parts, w, k, q_occ_max, 10)
+    mho = [max(m for _, m in streaks(s, contigs, w, k, q_occ_max, 10)) for s in stk]
+    assert mho[:2] == [128, 129] and mho[2] > 150, mho
+    check_case(L, ctx, contigs, stk, w=w, k=k, mid_occ=q_occ_max, q_occ_frac=0.0, occ_dist=10)

@@ -44,3 +44,10 @@ def test_emulated_seed_stage_long_reads(emu):
     assert max(SC.n_minimizers(r, cfg["w"], 15, cfg["mid_occ"], cfg["q_occ_frac"]) for r in reads) > 2048
     st = SC.check_case(L, ctx, contigs, reads, **cfg)
     assert st["anchors"] > 500 and st["big"] >= 3
+
+
+def test_emulated_seed_stage_capacity_edges(emu):
+    """2048 / 2049 minimizers in both query-side filter kernels and in select_kernel, q_occ_max / q_occ_max + 1 minimizers, and streaks
+    at the 128-entry heap's cap (see seed_check.check_edges)"""
+    L, ctx = emu
+    SC.check_edges(L, ctx)

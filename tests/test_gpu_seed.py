@@ -51,3 +51,11 @@ def test_seed_stage_wide_keys(dev):
     reads = synth.make_reads([seg], 40, 4000, 0.08, 63) + [bytes(seg[1000:9000]) * 2]  # the tandem read has equal keys
     st = SC.check_case(L, ctx, contigs, reads, mid_occ=20)
     assert st["wide"] >= 40 and st["ties"] >= 1
+
+
+@pytest.mark.parametrize("seed", [3, 4])
+def test_seed_stage_capacity_edges(dev, seed):
+    """2048 / 2049 minimizers in both query-side filter kernels and in select_kernel, q_occ_max / q_occ_max + 1 minimizers, and streaks
+    at the 128-entry heap's cap (see seed_check.check_edges)"""
+    L, ctx = dev
+    SC.check_edges(L, ctx, seed=seed)
