@@ -391,22 +391,24 @@ def read_parts(L, fn, w, k, is_hpc, mini_batch_size, batch_size, tmp_path):
     """every part mm_idx_reader_read of L makes of fn, in canonical form; the multi-part file the reader writes as it goes (-d) must
     hold the same parts"""
     from minimap2_b200.api import IdxOpt
-    L.mm_idx_reader_open.restype = C.c_void_p
-    L.mm_idx_reader_open.argtypes = [C.c_char_p, C.POINTER(IdxOpt), C.c_char_p]
-    L.mm_idx_reader_read.restype = C.c_void_p
-    L.mm_idx_reader_read.argtypes = [C.c_void_p, C.c_int]
-    L.mm_idx_reader_close.argtypes = [C.c_void_p]
+    # private function objects (L[name] makes a new one): the attributes of L keep the types minimap2_b200.api gives them
+    reader_open, reader_read, reader_close = L["mm_idx_reader_open"], L["mm_idx_reader_read"], L["mm_idx_reader_close"]
+    reader_open.restype = C.c_void_p
+    reader_open.argtypes = [C.c_char_p, C.POINTER(IdxOpt), C.c_char_p]
+    reader_read.restype = C.c_void_p
+    reader_read.argtypes = [C.c_void_p, C.c_int]
+    reader_close.argtypes = [C.c_void_p]
     io = IdxOpt(k=k, w=w, flag=MM_I_HPC if is_hpc else 0, bucket_bits=BUCKET_BITS, mini_batch_size=mini_batch_size, batch_size=batch_size)
-    rd = L.mm_idx_reader_open(str(fn).encode(), C.byref(io), str(tmp_path / "all.mmi").encode())
+    rd = reader_open(str(fn).encode(), C.byref(io), str(tmp_path / "all.mmi").encode())
     assert rd
     out = []
     while True:
-        mi = L.mm_idx_reader_read(rd, 1)
+        mi = reader_read(rd, 1)
         if not mi:
             break
         out += parse_mmi(dump(L, mi, tmp_path / "part.mmi"))
         L.mm_idx_destroy(mi)
-    L.mm_idx_reader_close(rd)
+    reader_close(rd)
     d = [c.digest() for c in parse_mmi(open(tmp_path / "all.mmi", "rb").read())]  # what `-d` writes: the parts back to back
     assert d == [c.digest() for c in out]
     return out

@@ -17,14 +17,13 @@ def setup(L):
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64]
 
 
-def device_seeds(L, ctx, mi, reads, flag, mid_occ, q_occ_frac, max_max_occ, occ_dist):
+def device_seeds(L, ctx, mi, reads, flag, mid_occ, q_occ_frac, max_max_occ, occ_dist, a_cap=4_000_000):
     n = len(reads)
     off = np.zeros(n + 1, dtype=np.int64)
     for i, s in enumerate(reads):
         off[i + 1] = off[i] + len(s)
     buf = np.frombuffer(b"".join(reads) + b"\0", dtype=np.uint8)
     a_off = np.zeros(n + 1, dtype=np.int64); rep = np.zeros(n, dtype=np.int32); nmini = np.zeros(n, dtype=np.int32)
-    a_cap = 4_000_000
     a = np.zeros((a_cap, 2), dtype=np.uint64); mp = np.zeros(int(off[-1]) + 16, dtype=np.uint64)
     tot = L.mmb_seed_batch_host(ctx, mi, n, buf.ctypes.data, off.ctypes.data, flag, mid_occ, q_occ_frac, max_max_occ, occ_dist,
                                 a_off.ctypes.data, rep.ctypes.data, nmini.ctypes.data, a.ctypes.data, a_cap, mp.ctypes.data, len(mp))
@@ -36,7 +35,8 @@ def device_seeds(L, ctx, mi, reads, flag, mid_occ, q_occ_frac, max_max_occ, occ_
     return out
 
 
-def check_case(L, ctx, contigs, reads, w=10, k=15, flag=0, mid_occ=10, q_occ_frac=0.01, max_max_occ=4095, occ_dist=500, is_hpc=0):
+def check_case(L, ctx, contigs, reads, w=10, k=15, flag=0, mid_occ=10, q_occ_frac=0.01, max_max_occ=4095, occ_dist=500, is_hpc=0, keep=None):
+    """keep: a list that receives the oracle's anchors of every read"""
     names = ["chr%d" % i for i in range(len(contigs))]
     seqs = [bytes(c) for c in contigs]
     arr = (C.c_char_p * len(seqs))(*seqs); nm = (C.c_char_p * len(seqs))(*[x.encode() for x in names])
@@ -53,6 +53,8 @@ def check_case(L, ctx, contigs, reads, w=10, k=15, flag=0, mid_occ=10, q_occ_fra
         assert ga.shape == ea.shape, (i, ga.shape, ea.shape)
         assert (ga == ea).all(), (i, int(np.argmax((ga != ea).any(axis=1))))
         stats["anchors"] += len(ea)
+        if keep is not None:
+            keep.append(ea)
         if len(ga):  # sort keys that differ in more than 33 bit positions: the radix kernels leave such reads to sort_block_kernel
             stats["wide"] += int(bin(int(np.bitwise_or.reduce(ga[:, 0] ^ ga[0, 0]))).count("1") > 33)
         if len(ea) > 64:

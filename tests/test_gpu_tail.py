@@ -49,15 +49,28 @@ def test_tail_matches_reference_vectors(ctx):
     assert not bad, bad[:10]
 
 
-def test_tail_long_hit(ctx):  # one hit of read scale: ~40 pieces, thousands of operations
+def test_tail_long_hit(ctx):
+    """hits of read scale: ~40 pieces and thousands of operations; and hits of a megabase read, with thousands of pieces and more than
+    65,535 operations (stage 1's 32-piece groups and stage 2's 32-operation chunks carry state thousands of times), one of them
+    without empty operations, all in one launch with short hits"""
     import minimap2_b200 as mb
     rng = np.random.default_rng(79)
-    big = []
-    for _ in range(8):
-        parts = [T.make_case(rng, low_complexity=False) for _ in range(40)]
+
+    def stitched(n_parts, low_complexity, no_empty=False):
+        parts = []
+        while len(parts) < n_parts:
+            p = T.make_case(rng, low_complexity=low_complexity)
+            if not (no_empty and any((int(w) >> 4) == 0 for pc in p["pieces"] for w in pc)):
+                parts.append(p)
         q = np.concatenate([p["qseq"] for p in parts]); t = np.concatenate([p["tseq"] for p in parts])
         pieces = [np.concatenate(p["pieces"]) if p["pieces"] else np.zeros(0, np.uint32) for p in parts]
-        big.append(dict(read=q, rev=0, qs=0, qseq=q, tseq=t, target=np.concatenate([t, np.zeros(16, np.uint8)]), t0=0, pieces=pieces, qspan=len(q), tspan=len(t)))
-    got = T.run_device(ctx, mb.lib(), big)
-    for g, c in zip(got, big):
-        assert T.same(g, T.run_oracle(c))
+        return dict(read=q, rev=0, qs=0, qseq=q, tseq=t, target=np.concatenate([t, np.zeros(16, np.uint8)]), t0=0, pieces=pieces, qspan=len(q), tspan=len(t))
+    big = [stitched(40, False) for _ in range(8)]
+    huge = [stitched(7000, True), stitched(7600, False, no_empty=True)]
+    short = [T.make_case(rng) for _ in range(64)]
+    cases = short[:32] + huge[:1] + short[32:] + huge[1:] + big
+    got = T.run_device(ctx, mb.lib(), cases)
+    for i, (g, c) in enumerate(zip(got, cases)):
+        e = T.run_oracle(c)
+        assert T.same(g, e), (i, len(c["pieces"]), e["n_cigar"])
+    assert all(len(c["pieces"]) >= 2000 and T.run_oracle(c)["n_cigar"] > 65535 for c in huge)
